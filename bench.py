@@ -1,16 +1,16 @@
 #!/usr/bin/env python
-"""Benchmark of the north-star hot path (rollout-collect -> buffer -> learn()) on B200.
+"""Benchmark of the north-star hot path (rollout-collect -> buffer -> learn()) on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config NAME]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config NAME] [--dump-outputs DIR]
 
-`--config` selects one of BASELINE.json's configurations; the default (what the driver runs) is configs[1]:
+`--config` selects one of BASELINE.json's configurations; the default is configs[1]:
 
   ppo_cartpole    configs[1]  PPO CartPole, 4096 batched envs/GPU, T=128, minibatch 256/GPU, 3 epochs (weak scaling)
   ppo_continuous  configs[4]  PPO continuous obs 11 / act 3 (Hopper dimensions, synthetic dynamics), 8192 envs IN TOTAL,
                               T=2048, 10 epochs, global minibatch 2048 (<= 512 per GPU), Adam 3e-4 (strong scaling)
   rainbow_frames  configs[2]  Rainbow (C51+PER+n-step+Noisy, CNN) on synthetic 84x84x4 uint8 frames, 1M-slot HBM replay
   apex            configs[3]  Ape-X DQN (dueling CNN), 256 actors -> PER sharded over the ranks (32 actors + 250k slots per GPU
-                              at 8 GPUs), RMSprop centred, gradient all-reduce
+                              at 8 GPUs; at most 1M slots = 56 GB of frames per 80 GB GPU), RMSprop centred, gradient all-reduce
 
 A "step" = one full iteration of the path on every rank:
   PPO      collect T steps of all envs (policy forward + sampling + physics + rollout write, all on the GPU), then learn():
@@ -21,10 +21,15 @@ A "step" = one full iteration of the path on every rank:
 reference-shaped plugin API (agent.act / env.step / agent.interact_callback / agent.process) with HOST numpy buffers,
 every host<->device copy inside the timed region.
 
+`--dump-outputs DIR` writes, right after the timed steps, what the last timed step computed (rollout / learn() results and
+the parameters it left) as DIR/<name>.npy in float32 / float64, at most 64 MB in all: an array above 1 Mi elements is
+replaced by a fixed, seeded sample of 1 Mi of its elements (flattened, the same positions in every run).  Inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
+
 `--impl reference` times the reference's CPU algorithm for the same path on the host cores (the oracle port: the
-reference is pure Python and /root/reference does not travel to the GPU box) on a BOUNDED SAMPLE of the workload: its own
-default worker count (8 actors; 1 for the replay agents), NOT the GPU arm's env count.  Its `config` is the GPU arm's
-(the contract: "on your arm's config"); `reference_sample`, `reference_actors` and `cpu_baseline.sample` say what ran.
+reference is pure Python) on a BOUNDED SAMPLE of the workload: its own default worker count (8 actors; 1 for the replay
+agents), NOT the GPU arm's env count.  Its `config` is the GPU arm's; `reference_sample`, `reference_actors` and
+`cpu_baseline.sample` say what ran.
 """
 import argparse
 import json
@@ -59,7 +64,12 @@ def parse():
     ap.add_argument("--epochs", type=int, default=None)
     ap.add_argument("--buffer", type=int, default=None)
     ap.add_argument("--rounds", type=int, default=None)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (float32/float64, <= 64 MB in all)")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
 
 
 def host_cores():
@@ -70,7 +80,7 @@ def host_cores():
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling (nvidia-smi queries every 200 ms during the timed window)
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -159,7 +169,7 @@ class PPOWorkload:
              "batch_size_per_gpu": self.B, "n_epoch": self.epochs, "hidden": self.H, "parallelism": f"dp{w}",
              "gradient_exchange": "none (1 GPU)" if w == 1 else
              "in-kernel reduce-scatter + all-gather over NVLink peer memory, once per minibatch step (csrc/ppo_fused.cu, core/parallel.py)",
-             "l2": "flushed between timed steps (256 MB fill, > 126 MB L2); every step re-collects its rollout"}
+             "l2": "flushed between timed steps (256 MB fill, > 50 MB L2); every step re-collects its rollout"}
         if self.override:
             c["override"] = True
         return c
@@ -195,6 +205,11 @@ class PPOWorkload:
         self.agent.learning_rate_decay(self.step_no)
         return res
 
+    def outputs(self):
+        ro = self.col.rollout
+        return {"rollout_state": ro.state, "rollout_action": ro.action, "rollout_reward": ro.reward, "rollout_done": ro.done,
+                "rollout_last_next_state": ro.last_next_state, "params": self.agent.network.flat}
+
     def env_steps_per_step(self):
         return self.n_envs * self.T * self.world
 
@@ -225,24 +240,19 @@ class PPOWorkload:
                 times.append(a0.elapsed_time(a1))
         dur_ms = sum(times) / len(times)
         flops = float(n_run) * self.B * 6.0 * (self.D * self.H + self.H * self.H + self.H * self.nout)   # fwd + 2x bwd (SURVEY 8d)
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
         ach = flops / (dur_ms * 1e-3) / 1e12
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_ppo_epoch_kernel_traffic.json")))["dram_bytes_per_launch"]
-        except Exception:
-            pass
-        ffma = 148 * 128 * 2 * 1.965e-3
+        ffma = 132 * 128 * 2 * 1.98e-3                   # H100 SXM: 132 SMs x 128 FP32 FMA/clk x 1.98 GHz boost (data sheet 67)
         return {"kernel": f"ppo_epoch_kernel (persistent cooperative PPO minibatch loop, {n_run} steps/launch)", "bound": "tensor",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-                "traffic": traffic if (self.name == "ppo_cartpole" and n_run == 2048) else None,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400 (of fallback)",
+                "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else
+                                "H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)"),
                 "algorithmic_flops_per_launch": flops, "ms_per_launch": dur_ms, "us_per_minibatch_step": 1e3 * dur_ms / n_run,
                 "fp32_ffma_peak_tflops": ffma, "frac_of_fp32_ffma_peak": ach / ffma, "world": self.world,
                 "note": "one launch = one epoch slice of sequential minibatch steps (forward, loss, backward, clip, Adam"
                         + (", gradient exchange over NVLink" if self.world > 1 else "") + "); the step is latency / grid-barrier "
-                        "bound at the reference minibatch size (DESIGN.md 3b has the per-phase timeline); frac is against the "
-                        "measured bf16 tensor peak as the contract asks, frac_of_fp32_ffma_peak against 148 SMs x 128 FMA/clk x 1.965 GHz"}
+                        "bound at the reference minibatch size (DESIGN.md 3b); frac is against the bf16 tensor peak, "
+                        "frac_of_fp32_ffma_peak against 132 SMs x 128 FMA/clk x 1.98 GHz"}
 
     # ---- labelled scaled-minibatch variant (SURVEY 8d: "and a labelled scaled variant (e.g. 16 384)") ----------------
     def extra(self):
@@ -266,7 +276,7 @@ class PPOWorkload:
         ms = e0.elapsed_time(e1) / n
         big._graphs.clear()
         return {"label": "scaled minibatch variant, NOT the headline: same rollout (4096 envs x T=128), minibatch 16384, 3 epochs x 32 "
-                         "steps through the CUDA-graph path (tcgen05 forward GEMM + FFMA backward tiles)",
+                         "steps through the CUDA-graph path (wgmma forward GEMM + FFMA backward tiles)",
                 "batch_size": B2, "ms_per_step": ms, "env_steps_per_sec": self.n_envs * self.T / (ms * 1e-3),
                 "learner_transitions_per_sec": self.n_envs * self.T * self.epochs / (ms * 1e-3)}
 
@@ -403,7 +413,8 @@ class ReplayWorkload:
             self.agent_name = "rainbow"
         else:
             # config/ape_x/atari.py:16-40,53-55 with num_workers = 256
-            self.n_actors, self.buffer, self.n_step, self.update_period = 256 // world, 2_000_000 // world, 3, 100
+            # the reference's 2M-slot replay, sharded; capped at 1M slots per GPU (56 GB of uint8 frames on an 80 GB H100)
+            self.n_actors, self.buffer, self.n_step, self.update_period = 256 // world, min(2_000_000 // world, 1_000_000), 3, 100
             self.B = 512 // world
             self.scaling = "strong"
             self.agent_kw = dict(network="dueling", alpha=0.6, beta=0.4, learn_period=4, uniform_sample_prob=1e-3, clip_grad_norm=40.0,
@@ -470,6 +481,9 @@ class ReplayWorkload:
             res = r or res
         return res
 
+    def outputs(self):
+        return {"params": self.agent.network.flat}
+
     def env_steps_per_step(self):
         return self.n_actors * self.update_period * self.rounds * self.world
 
@@ -501,15 +515,15 @@ class ReplayWorkload:
             fc = 2.0 * (2 * 3136 * 512 + 512 * self.A + 512)
         fwd = conv + fc
         flops = self.B * fwd * (3 + 2)                                # 3 forwards (s online, s' online, s' target) + backward = 2 forwards
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
         ach = flops / (ms * 1e-3) / 1e12
-        return {"kernel": "learn() of one minibatch: im2col + FFMA tile GEMMs (conv lowering, csrc/conv.cu + csrc/linear.cu) dominate; "
-                          "per-kernel shares in profiles/r02_kernels.md", "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-                "frac": ach / peak, "traffic": None,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400 (of fallback)",
+        return {"kernel": "learn() of one minibatch: im2col + FFMA tile GEMMs (conv lowering, csrc/conv.cu + csrc/linear.cu) dominate",
+                "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
+                "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else
+                                "H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)"),
                 "algorithmic_flops_per_launch": flops, "ms_per_learn": ms, "learner_transitions_per_sec_learn_only": self.B / (ms * 1e-3),
                 "replay_gather_bytes_per_learn": self.B * (2 * 28224 + 8 * self.n_step + 8), "world": self.world,
-                "note": "latency-bound at B=" + str(self.B) + ": ~60 launches per learn(); fp32 FFMA tiles, not tcgen05, for the minibatch-sized GEMMs"}
+                "note": "latency-bound at B=" + str(self.B) + ": ~60 launches per learn(); fp32 FFMA tiles, not wgmma, for the minibatch-sized GEMMs"}
 
     def extra(self):
         return None
@@ -735,6 +749,11 @@ class ACWorkload:
             res = r or res
         return res
 
+    def outputs(self):
+        out = {"actor_params": self.agent.actor.flat}
+        out.update({f"critic{i + 1}_params": c.flat for i, c in enumerate(self.agent.critics)})
+        return out
+
     def env_steps_per_step(self):
         return self.n_actors * self.update_period * self.rounds * self.world
 
@@ -765,11 +784,12 @@ class ACWorkload:
         actor = 2.0 * (D * H + H * H + H * 2 * A)
         critic = 2.0 * (D * H + A * H + 2 * H * H + H)
         flops = self.B * (4 * actor + 12 * critic)
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
         ach = flops / (ms * 1e-3) / 1e12
         return {"kernel": "SAC.learn() of one minibatch: fp32 FFMA tile GEMMs (csrc/linear.cu) + the row kernels of csrc/actor_critic.cu",
                 "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400 (of fallback)",
+                "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else
+                                "H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)"),
                 "algorithmic_flops_per_launch": flops, "ms_per_learn": ms, "learner_transitions_per_sec_learn_only": self.B / (ms * 1e-3),
                 "world": self.world, "cuda_graph": bool(agent._graphs),
                 "note": f"latency-bound at B={self.B}: ~83 kernels of <= 0.5 GFLOP each per learn(), "
@@ -881,11 +901,11 @@ def args_config_is_ppo(wl):
 
 
 def best_cpu_threads(wl, workers):
-    """The reference is torch-eager with tiny (batch-1 / minibatch) ops: more intra-op threads than the box can really
+    """The reference is torch-eager with tiny (batch-1 / minibatch) ops: more intra-op threads than the host can really
     schedule make it SLOWER.  To time the reference at its best, try a few thread counts on one short rollout each."""
     avail = host_cores()
-    # 1 thread and "all cores" are both far from the optimum for these op sizes (measured: 1 -> 20x slower, 128 -> 200x
-    # slower than 8 on the GPU box's host) and would eat minutes of a bounded baseline: sweep the plausible range only
+    # 1 thread and "all cores" are both far from the optimum for these op sizes (an order of magnitude or more slower than 8)
+    # and would eat minutes of a bounded baseline: sweep the plausible range only
     cands = sorted({c for c in ((4, 8, 16) if args_config_is_ppo(wl) else (8, 16, 32)) if 1 <= c <= avail}) or [min(avail, 4)]
     best, best_rate, tried = cands[0], 0.0, {}
     for c in cands:
@@ -919,6 +939,28 @@ def run_reference(args, rank):
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 20                    # elements kept of a larger output array
+DUMP_LIMIT = 64 * 1024 * 1024            # bytes over all files
+
+
+def dump_outputs(path, wl, res, np):
+    """The last timed step's outputs (wl.outputs() tensors, numeric entries of the step's result dict) as .npy files."""
+    import numbers
+    arrays = {k: v.detach().float().reshape(-1).cpu().numpy() for k, v in wl.outputs().items()}
+    arrays.update({f"result_{k}": np.asarray(v, dtype=np.float64) for k, v in (res or {}).items()
+                   if isinstance(v, numbers.Real)})
+    for k, a in arrays.items():
+        if a.size > DUMP_SAMPLE:
+            arrays[k] = a[np.sort(np.random.RandomState(0).choice(a.size, DUMP_SAMPLE, replace=False))]
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed {DUMP_LIMIT}")
+    os.makedirs(path, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(path, f"{k}.npy"), a)
+
+
+# ------------------------------------------------------------------------------------------------
 def main():
     args = parse()
     rank = int(os.environ.get("RANK", 0))
@@ -943,6 +985,7 @@ def main():
         if rank == 0 or trace_all:
             print(f"[bench {time.strftime('%H:%M:%S')} r{rank}] {msg}", file=sys.stderr, flush=True)
 
+    torch.manual_seed(0)           # network initialisation and minibatch permutations: the same inputs in every run
     wl = make_workload(args.config, args, world)
     log(f"world={world} config={args.config}: build")
     wl.build(torch, dev, rank)
@@ -969,6 +1012,8 @@ def main():
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl, res, np)
     t = torch.tensor([ms], dtype=torch.float64, device=dev)
     if world > 1:
         dist.barrier()

@@ -1,4 +1,4 @@
-/* jorldy_b200 — C ABI of the B200-native rollout-collect -> buffer -> learn() core.
+/* jorldy_b200 — C ABI of the H100-native rollout-collect -> buffer -> learn() core.
  *
  * The reference (kakaoenterprise/JORLDY) is pure Python and has no FFI of its own; its plugin
  * boundary is the Python classes Agent / Env / Buffer / Network / Optimizer.  This header is the
@@ -91,7 +91,7 @@ JB_API int jb_gemm(const float* A, int lda, int a_kc, const float* B, int ldb, i
                    float* rowsum_a, int accumulate, void* stream);
 JB_API int jb_linear_fwd(const float* x, const float* w, const float* b, float* y, int M, int in_f, int out_f,
                          int relu, void* stream);
-/* tcgen05 / TMEM 3xTF32 forward for large M (M % 128 == 0, out_f % 128 == 0, in_f % 32 == 0); -22 otherwise */
+/* wgmma 3xTF32 forward for large M (M % 128 == 0, out_f % 128 == 0, in_f % 32 == 0); -22 otherwise */
 JB_API int jb_linear_fwd_tc(const float* x, const float* w, const float* b, float* y, int M, int in_f, int out_f,
                             int relu, void* stream);
 JB_API int jb_linear_bwd_dx(const float* dy, const float* w, float* dx, int M, int in_f, int out_f,

@@ -26,7 +26,7 @@ typedef struct jb_ppo_fused_args {
   float *headp;                      /* [H/32, 2, B, 4] per-column-tile partial head outputs */
   float *h2t;                        /* [H/32, B, 32] tiled copy of h2 */
   float *W2t;                        /* [H/32, H, 32] tiled shadow of W2 (maintained by the Adam phase) */
-  float *W2img;                      /* [2 (hi | lo), H/32, H/32, 32 x 32] UMMA-layout images of W2 for the tensor-core
+  float *W2img;                      /* [2 (hi | lo), H/32, H/32, 32 x 32] wgmma-layout (K-major, 128-byte swizzle) images of W2 for the tensor-core
                                       * forward phase (3xTF32 split), maintained by the Adam phase; NULL: FFMA tiles only */
   float *W2Timg;                     /* [2, H/128, H/32, 128 x 32] the same for W2^T (operand of the tensor-core dh1 jobs) */
   float *partials;                   /* [256] per-CTA squared-norm partials */

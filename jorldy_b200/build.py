@@ -1,4 +1,4 @@
-"""Builds libjorldy_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libjorldy_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 No torch involvement: the library is plain CUDA runtime + extern "C" entry points declared in
 include/jorldy_b200.h.  Objects are cached under jorldy_b200/lib/obj and rebuilt when a source
@@ -16,7 +16,7 @@ OBJDIR = os.path.join(LIBDIR, "obj")
 LIB = os.path.join(LIBDIR, "libjorldy_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

@@ -18,7 +18,7 @@ def require_cuda(device):
     device = torch.device(device) if device is not None else torch.device("cuda")
     if device.type != "cuda":
         raise JbError(
-            f"jorldy_b200 runs its hot path only on CUDA (sm_100a); got device '{device}'. "
+            f"jorldy_b200 runs its hot path only on CUDA (sm_90a); got device '{device}'. "
             "There is no CPU fallback — use the reference (or oracle/) for CPU runs.")
     if not torch.cuda.is_available():
         raise JbError("CUDA is not available: jorldy_b200 has no CPU fallback.")

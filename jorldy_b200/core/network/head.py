@@ -106,9 +106,9 @@ class CNNHead:
             Mr = M * oh * ow
             col = net._buf(f"{tag}head.col{li}", (Mr, K))
             # conv weight gradients are [co, ci k k] = a few 32 x 32 tiles contracted over M * oh * ow rows: split the
-            # contraction over the grid (148 SMs) and fold the partials in a fixed order
+            # contraction over the grid (two waves of the 132 SMs) and fold the partials in a fixed order
             tiles = ((K + 31) // 32) * ((co + 31) // 32)
-            splits = min(64, max(1, 296 // tiles), max(1, Mr // 512))
+            splits = min(64, max(1, 264 // tiles), max(1, Mr // 512))
             ws = net._buf(f"{tag}head.dwws{li}", (splits * (co * K + co),)) if splits > 1 else None
             C.jb_linear_bwd_dw_splitk(ptr(dy), ptr(col), ptr(net.g[f"head.{name}.weight"]), ptr(net.g[f"head.{name}.bias"]),
                                       Mr, K, co, ptr(ws), splits, s)

@@ -4,12 +4,12 @@ from ..dev import C, ptr, stream_ptr
 
 import os
 
-TC_MIN_ROWS = 1024     # below this a 128x128 tile grid cannot fill the 148 SMs: stay on the fp32 FFMA tiles
+TC_MIN_ROWS = 1024     # below this a 128x128 tile grid cannot fill the 132 SMs: stay on the fp32 FFMA tiles
 _USE_TC = os.environ.get("JB_NO_TC", "0") != "1"
 
 
 def linear_fwd(x, w, b, y, relu):
-    """y = act(x W^T + b).  Large-M products (env-row batches) go to the tcgen05/TMEM 3xTF32 kernel
+    """y = act(x W^T + b).  Large-M products (env-row batches) go to the wgmma 3xTF32 kernel
     (csrc/tc_gemm.cu); minibatch-sized ones to the fp32 FFMA tiles (csrc/linear.cu)."""
     M, in_f = x.shape
     out_f = w.shape[0]

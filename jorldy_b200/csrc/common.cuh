@@ -1,4 +1,4 @@
-// Shared device/host helpers for the jorldy_b200 sm_100a kernels.
+// Shared device/host helpers for the jorldy_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 #define JB_ERR_INVALID (-22)   /* EINVAL-style: bad argument */
 #define JB_ERR_CUDA (-5)       /* EIO-style: CUDA launch / runtime failure */
 
-#define JB_SM_COUNT 148        /* B200: 2 dies x 74 SMs */
+#define JB_SM_COUNT 132        /* H100 SXM */
 
 #define JB_API extern "C" __attribute__((visibility("default")))
 
@@ -19,7 +19,7 @@ static inline int jb_check_launch() {
 static inline int jb_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // Persistent-style grid size: enough CTAs to cover `work` items at `per_cta`
-// items each, rounded up to whole waves of the 148 SMs, capped at `max_waves`.
+// items each, rounded up to whole waves of the 132 SMs, capped at `max_waves`.
 static inline int jb_grid_for(long long work, int per_cta, int max_waves = 32) {
   long long ctas = (work + per_cta - 1) / per_cta;
   if (ctas < 1) ctas = 1;

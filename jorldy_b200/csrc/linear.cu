@@ -15,7 +15,7 @@
 // Two instantiations:
 //   * "small"  32x32 tile, 4x4 micro-tile, 4-way in-CTA split-K (256 threads): the minibatch
 //     products (M = 32..2048 rows) are only a few hundred tiles, so a CTA must be a small tile
-//     to cover the 148 SMs; the in-CTA k split keeps 8 warps resident for latency hiding and
+//     to cover the 132 SMs; the in-CTA k split keeps 8 warps resident for latency hiding and
 //     is reduced through shared memory in a fixed order.
 //   * "large"  128x64 tile, 8x4 micro-tile (256 threads) for the act()/pre-pass products
 //     (M = thousands of env rows).
@@ -388,7 +388,7 @@ template <bool A_KC, bool B_KC>
 int launch_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
                 const float* bias, int relu, const float* mask, int ldmask, float* rowsum_a, int accumulate,
                 cudaStream_t s) {
-  // small-tile kernel while a 128x64 tiling would leave most of the 148 SMs idle
+  // small-tile kernel while a 128x64 tiling would leave most of the 132 SMs idle
   const long long big_tiles = (long long)jb_div_up(M, 128) * jb_div_up(N, 64);
   if (big_tiles >= 2 * JB_SM_COUNT) {
     dim3 grid(jb_div_up(N, 64), jb_div_up(M, 128));

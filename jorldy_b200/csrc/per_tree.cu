@@ -8,7 +8,7 @@
 //   :70-101 sample (uniform/prioritised split, IS weights, stats) -> jb_per_sample
 //
 // Tree layout is the reference's: tree_size = 2N-1, root at 0, children 2i+1 / 2i+2, leaves at
-// N-1 .. 2N-2, float64.  (1 M slots -> 16 MB, 2 M -> 32 MB: L2-resident on B200's 126 MB L2.)
+// N-1 .. 2N-2, float64.  (1 M slots -> 16 MB, 2 M -> 32 MB: L2-resident in H100's 50 MB L2.)
 //
 // Bit-exactness of the incremental-delta tree (SURVEY hard part 2): the reference applies a
 // batch of B updates one after another, each adding delta_i = new_i - old_i to every ancestor.

@@ -3,10 +3,9 @@
 //
 // Why: at the reference's minibatch size (256 x [4-512-512-(A+1)]) one step is ~0.4 GFLOP and < 4 MB of
 // traffic, i.e. microseconds of work, and one learn() is n_epoch * N*T/B = 6144 strictly sequential
-// steps.  As 13 separate launches per step (the "graph" path) each step cost 71 us, almost all of it
-// launch gaps and cold per-kernel load latency (profiles/r01_launches_ppo_summary.md).  Here one CTA per
-// SM stays resident for the whole epoch and a step is THREE phases separated by a hand-rolled grid
-// barrier (~1.3 us each; scripts/bench_gridbar.cu compares the variants):
+// steps.  As 13 separate launches per step (the "graph" path) almost all of a step is launch gaps and
+// cold per-kernel load latency.  Here one CTA per SM stays resident for the whole epoch and a step is
+// THREE phases separated by a hand-rolled grid barrier (scripts/bench_gridbar.cu compares the variants):
 //
 //   P1  layer-2 forward tiles (32x32, fp32 FFMA, 16-way in-CTA split-K).  The A panel h1 = relu(x W1^T + b1)
 //       is GENERATED in shared memory from the gathered state rows (K = D <= 16), never read from HBM; the
@@ -44,9 +43,8 @@
 //     rank's norm table;
 //   * every CTA reads its Adam slice of the averaged gradient and all chunk norms as they arrive, folds the norms in a
 //     fixed order (identical bits on all ranks) and applies clip + Adam.
-//   Measured history at 2 GPUs (profiles/r02_exchange.md): flag + fence protocols cost 3.5-6 us PER HOP (release store or
-//   system fence waiting for remote write acknowledgements; acquire polls), 64-72 us per step; un-throttled relaxed polling
-//   of flags saturated L2 (93 us).
+//   Flag + fence protocols were slower: every hop paid a release store or system fence waiting for remote write
+//   acknowledgements plus acquire polls, and un-throttled relaxed polling of flags saturated L2.
 //   * the two scalar means of critic_loss = max(mean, mean) (ppo.py:151-154) are GLOBAL: each rank sends its two row sums to
 //     the peers during the row phase (two LL words); receiving step s's message from a peer also proves that the peer has
 //     finished step s-1.
@@ -57,6 +55,7 @@
 #include <cstdlib>
 #include "common.cuh"
 #include "ppo_rowmath.cuh"
+#include "wgmma.cuh"
 #include "../../include/jorldy_b200_fused.h"
 
 namespace {
@@ -324,39 +323,14 @@ __device__ __forceinline__ float4 dh2_quad(const float* drow, const float4 (&wr)
   return make_float4(hv.x > 0.f ? t.x : 0.f, hv.y > 0.f ? t.y : 0.f, hv.z > 0.f ? t.z : 0.f, hv.w > 0.f ? t.w : 0.f);
 }
 
-// ---- tcgen05 building blocks for the tensor-core forward phase (same descriptors as csrc/tc_gemm.cu) -----------------
-// Operand tiles live in shared memory in the UMMA canonical K-major SWIZZLE_128B layout: one 128-byte row (32 fp32 of K)
-// per tile row, eight rows per 1 KB atom, 16-byte chunk index XOR row-in-atom.
-__device__ __forceinline__ unsigned tc_tile_off(int row, int chunk) { return (unsigned)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
-__device__ __forceinline__ unsigned long long tc_desc(unsigned smem_addr) {
-  unsigned long long d = 0;
-  d |= (unsigned long long)((smem_addr >> 4) & 0x3FFF);        // start address
-  d |= (unsigned long long)1 << 16;                            // leading byte offset (unused: swizzled K-major)
-  d |= (unsigned long long)((1024 >> 4) & 0x3FFF) << 32;       // stride byte offset: 1 KB between 8-row atoms
-  d |= (unsigned long long)1 << 46;                            // descriptor version (sm_100)
-  d |= (unsigned long long)2 << 61;                            // SWIZZLE_128B
-  return d;
-}
-// instruction descriptor: D = F32, A = B = TF32, both K-major, M = 128, N = 32
-constexpr unsigned TC_IDESC_N32 = (1u << 4) | (2u << 7) | (2u << 10) | ((32u >> 3) << 17) | ((128u >> 4) << 24);
-__device__ __forceinline__ void tc_mma(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc, unsigned accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit(unsigned mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(mbar) : "memory");
-}
+// ---- tensor-core phases (TC instantiation): 3xTF32 wgmma products, building blocks in csrc/wgmma.cuh ----------------
+using jbwg::tile_off;
 __device__ __forceinline__ void mbar_init(unsigned mbar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(mbar), "r"(count) : "memory");
 }
 // Bounded: a tensor-core pipeline bug must fail the launch (trap -> CUDA error on the host), never hang the GPU.  The
 // bound is counted in SM clock cycles (clock64 is a register read; %globaltimer costs microseconds per read, which made
-// every wait that missed its first try a 2-5 us stall).
+// every wait that missed its first try a multi-microsecond stall).
 __device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
   unsigned done = 0;
   const long long t0 = clock64();
@@ -388,9 +362,10 @@ __device__ __forceinline__ float tf32_lo(float x) {
 constexpr int TC_A_BYTES = 2 * 128 * 128;        // one A chunk: hi | lo, each [128 rows][32 k] fp32 = 16 KB
 constexpr int TC_B_BYTES = 2 * 32 * 128;         // one B chunk: hi | lo, each [32 rows][32 k] fp32 = 4 KB
 constexpr int TC_NA = 3, TC_NB = 5;              // ring depths: A chunks are generated, B chunks stream in 4 ahead (+ 8 KB: x tile)
-constexpr int TC_BAR_WORD = 1664;                // s_small word offset of the tensor-core mbarriers (32 x 8 bytes)
-constexpr int TC_TMEM_WORD = 1660;               // s_small word that receives the TMEM base address
-constexpr int TC_NBAR = 24;                      // [0..9] forward, [10..15] dh1 jobs, [16..23] dW2 jobs
+constexpr int TC_BAR_WORD = 1664;                // s_small word offset of the tensor-core mbarriers (8 x 8 bytes)
+constexpr int TC_BAR_JB = TC_NB;                 // [0..4] forward B chunk landed, [5..7] dh1 jobs' W2^T chunk landed
+constexpr int TC_NBAR = TC_NB + TC_NA;
+constexpr int TC_LD = 36;                        // row stride (floats) of the [128][32] accumulator image the epilogues read
 
 // timing trace (debug; JB_FUSED_SKIP bit 8): clock64 at fixed points of the LAST step, per CTA, 32 slots
 __device__ long long g_trace[256 * 48];
@@ -418,16 +393,17 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
   stp.init(s_small + 1058);                    // 8-byte mbarrier: parameter stash
   float* dvs = s_small + 1088;                 // [MAX_B] second candidate value-head gradient of every row (P3); norm partials (P5)
   float* hb = s_small + 1600;                  // [MAXO] head biases
-  // tensor-core forward phase (TC instantiation): operand rings inside R0..R1 (1 KB aligned), 10 mbarriers
-  // ([0..2] A chunk retired, [3..8] B chunk landed, [9] tile accumulated), 32 TMEM columns for the whole launch
-  unsigned tc_base = 0, tc_tmem = 0, tc_tiles = 0;
+  // tensor-core phases (TC instantiation): operand rings inside R0..R1 (1 KB aligned), TC_NBAR mbarriers for the bulk
+  // copies; each warpgroup keeps its 64 x 32 accumulator in registers (csrc/wgmma.cuh)
+  unsigned tc_base = 0;
   unsigned long long tc_g = 0;                 // chunks issued so far by this CTA: ring positions and mbarrier phases
-  unsigned long long jb_g = 0;                 // same for the tensor-core dh1 jobs (mbarriers 10..15)
-  unsigned long long ja_g = 0;                 // ... and the dW2 jobs (mbarriers 16..18)
+  unsigned long long jb_g = 0;                 // same for the tensor-core dh1 jobs
+  unsigned long long ja_g = 0;                 // ... and the dW2 jobs
   const unsigned tc_bar = smem_u32(s_small + TC_BAR_WORD);
   float* tcp = nullptr;                        // generic pointer to the ring base (epilogue scratch)
+  float* tcs = nullptr;                        // [128][TC_LD] accumulator image for the epilogues (A ring slot 1)
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = tid >> 7;
   const unsigned int nctas = gridDim.x;
   const int cta = blockIdx.x;
   const int B = a.B, D = a.D, H = a.H, A = a.A, nout = a.nout;
@@ -442,18 +418,12 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
   if (TC) {
     tc_base = (smem_u32(R0) + 1023u) & ~1023u;
     tcp = R0 + ((tc_base - smem_u32(R0)) >> 2);
+    tcs = tcp + TC_A_BYTES / 4;
     if (tid == 0) {
       for (int i = 0; i < TC_NBAR; ++i) mbar_init(tc_bar + 8u * i, 1);
       asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
-    if (warp == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(s_small + TC_TMEM_WORD)), "r"(32u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    tc_tmem = *reinterpret_cast<volatile unsigned*>(s_small + TC_TMEM_WORD);
   }
   HeadTab& ht = *reinterpret_cast<HeadTab*>(s_small + 896);   // 32 pointers: shared memory, not 64 live registers
   if (tid == 0) {
@@ -491,9 +461,9 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       const int e = (int)(i - w2_lo) * 4, n = e / H, k = e - n * H;
       *reinterpret_cast<float4*>(&a.W2t[((size_t)(k >> 5) * H + n) * 32 + (k & 31)]) = v;
       if (TC) {
-        // UMMA-ready images of W2 (hi | lo of the 3xTF32 split): tile (n / 32, k / 32) = [32 rows][32 k] in the swizzled
+        // wgmma-ready images of W2 (hi | lo of the 3xTF32 split): tile (n / 32, k / 32) = [32 rows][32 k] in the swizzled
         // K-major layout, so that a B chunk of the forward phase is ONE 4 KB bulk copy per image
-        float* img = a.W2img + ((size_t)(n >> 5) * (H >> 5) + (k >> 5)) * 1024 + (tc_tile_off(n & 31, (k & 31) >> 2) >> 2);
+        float* img = a.W2img + ((size_t)(n >> 5) * (H >> 5) + (k >> 5)) * 1024 + (tile_off(n & 31, (k & 31) >> 2) >> 2);
         *reinterpret_cast<float4*>(img) = v;
         *reinterpret_cast<float4*>(img + (size_t)H * H) = make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w));
         // ... and of W2^T for the dh1 jobs: tile (k / 128, n / 32) = [128 rows k][32 columns n]
@@ -501,7 +471,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int kk = k + q;
-          float* t = a.W2Timg + ((size_t)(kk >> 7) * (H >> 5) + (n >> 5)) * 4096 + (tc_tile_off(kk & 127, (n & 31) >> 2) >> 2) + (n & 3);
+          float* t = a.W2Timg + ((size_t)(kk >> 7) * (H >> 5) + (n >> 5)) * 4096 + (tile_off(kk & 127, (n & 31) >> 2) >> 2) + (n & 3);
           t[0] = vv4[q];
           t[(size_t)H * H] = tf32_lo(vv4[q]);
         }
@@ -578,7 +548,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     // =========================== P1: h2 = relu(relu(x W1^T + b1) W2^T + b2), partial head outputs ========
     // parameter stash: ONE bulk request per tensor per CTA, issued from different warps.  (Per-thread loads of
     // W1 / b1 / b2 / head rows had every warp of every CTA hit the same few KB right after the barrier: > 500 K
-    // sector requests queued on ~100 L2 lines, 4-5 us before the first value arrived.)
+    // sector requests queued on ~100 L2 lines, microseconds before the first value arrived.)
     stp.bytes = (unsigned)(H * D + (2 + nout) * H) * 4u;
     stp.commit();                                  // thread 0 arrives with the byte count before anything else
     if (tid == 32) stp.copy(R2, a.W1, (unsigned)(H * D) * 4u);
@@ -600,17 +570,17 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     }
     if constexpr (TC) {
       // ---- tensor-core forward: one 128 (minibatch rows) x 32 (hidden units) tile per job, K = H in chunks of 32.
-      // A chunk = h1[128 rows][32 k] = relu(x W1^T + b1), GENERATED straight into the UMMA layout (hi | lo of the 3xTF32
-      // split) by all threads; B chunk = hi | lo image of W2[n0..n0+32][32 k] (kept current by the Adam phase), one 8 KB
-      // pair of bulk copies five chunks ahead; thread 0 issues 4 x 3 tcgen05.mma (M128 N32 K8, kind::tf32) per chunk into
-      // 32 TMEM columns and commits to the chunk's mbarrier, which is what lets the generators reuse the A slot.
+      // A chunk = h1[128 rows][32 k] = relu(x W1^T + b1), GENERATED straight into the swizzled K-major layout (hi | lo of
+      // the 3xTF32 split) by all threads; B chunk = hi | lo image of W2[n0..n0+32][32 k] (kept current by the Adam phase),
+      // one 8 KB pair of bulk copies four chunks ahead; each warpgroup issues 4 x 3 wgmma (m64n32k8, tf32) per chunk for its
+      // 64 rows and leaves them in flight while the next chunk is generated into another A slot.
       const int NKC = H >> 5;
       for (int job = cta; job < nJ1; job += (int)nctas) {
         const int mt = job / NTL, nt = job - mt * NTL, m0 = mt * 128, n0 = nt * 32;
         const int r = tid & 127, half = tid >> 7;
         auto issue_b = [&](int kc, unsigned long long g) {
           const unsigned slot = (unsigned)(g % TC_NB);
-          const unsigned bar = tc_bar + 8u * (3u + slot), dst = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES;
+          const unsigned bar = tc_bar + 8u * slot, dst = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES;
           mbar_expect_tx(bar, TC_B_BYTES);
           const float* src = a.W2img + ((size_t)nt * NKC + kc) * 1024;
           bulk_g2s(dst, src, 4096u, bar);
@@ -644,11 +614,11 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         __syncthreads();
         const float* W1s = R2;
         const float* b1s = PS + (MAXO + 1) * PK;
+        float acc[16];
         TR(1);
         for (int kc = 0; kc < NKC; ++kc) {
           const unsigned long long g = tc_g + kc;
-          const unsigned abuf = tc_base + (unsigned)(g % TC_NA) * TC_A_BYTES;
-          if (g >= TC_NA) mbar_wait(tc_bar + 8u * (unsigned)(g % TC_NA), (unsigned)((g / TC_NA - 1) & 1));   // chunk g - 3 retired
+          const unsigned abuf = tc_base + (unsigned)(g % TC_NA) * TC_A_BYTES;   // chunk g - 3's slot: retired (wait below)
           // generator: lane = hidden unit 32 kc + lane (its W1 row in registers), warp = rows 16 warp .. + 15
           const int k = kc * 32 + lane;
           float w1k[ND];
@@ -673,52 +643,42 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           for (int j = 0; j < 16; ++j) {
             const int row = warp * 16 + j;
             const float hi = fmaxf(hv[j] + b1k, 0.f);
-            const unsigned off = tc_tile_off(row, lane >> 2) + ((unsigned)(lane & 3) << 2);
+            const unsigned off = tile_off(row, lane >> 2) + ((unsigned)(lane & 3) << 2);
             asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(abuf + off), "f"(hi) : "memory");
             asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(abuf + 16384u + off), "f"(tf32_lo(hi)) : "memory");
             if (nt == 0) a.h1[((size_t)kc * B + m0 + row) * 32 + lane] = hi;                  // tiled [H/32][B][32]
           }
-          asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy stores -> async proxy (UMMA reads)
-          __syncthreads();
-          if (tid == 0) {
-            const unsigned slot = (unsigned)(g % TC_NB);
-            mbar_wait(tc_bar + 8u * (3u + slot), (unsigned)((g / TC_NB) & 1));            // B chunk landed
-            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-            const unsigned bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const unsigned ko = 32u * j;                                               // K = 8 tf32 = 32 bytes inside the swizzled row
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + ko), TC_IDESC_N32, (kc > 0 || j > 0) ? 1u : 0u);
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + 4096u + ko), TC_IDESC_N32, 1u);
-              tc_mma(tc_tmem, tc_desc(abuf + 16384u + ko), tc_desc(bbuf + ko), TC_IDESC_N32, 1u);
-            }
-            tc_commit(tc_bar + 8u * (unsigned)(g % TC_NA));
-            if (kc == NKC - 1) tc_commit(tc_bar + 8u * 9u);
-            if (kc + TC_NB - 1 < NKC) {              // refill the B ring: chunk kc + 5 goes where chunk kc - 1 lived
-              if (kc >= 1) mbar_wait(tc_bar + 8u * (unsigned)((g - 1) % TC_NA), (unsigned)(((g - 1) / TC_NA) & 1));
-              issue_b(kc + TC_NB - 1, g + TC_NB - 1);
-            }
-          }
+          jbwg::wait<0>();                                              // chunk g - 1's products of this warpgroup retired
+          jbwg::fence_acc(acc);
+          asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy stores -> async proxy (wgmma reads)
+          __syncthreads();                                              // ... and those of the other warpgroup
+          const unsigned slot = (unsigned)(g % TC_NB);
+          if (tid == 0 && kc + TC_NB - 1 < NKC) issue_b(kc + TC_NB - 1, g + TC_NB - 1);   // chunk kc + 4 where chunk kc - 1 lived
+          mbar_wait(tc_bar + 8u * slot, (unsigned)((g / TC_NB) & 1));   // B chunk landed
+          const unsigned bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES, aw = abuf + (unsigned)wg * 8192u;
+          jbwg::fence();
+          jbwg::mma3_n32(acc, aw, aw + 16384u, bbuf, bbuf + 4096u, kc == 0);
+          jbwg::commit();
         }
         TR(3);
-        // ---- epilogue: TMEM -> registers (warp w: lanes 32 (w & 3).., columns 16 (w >> 2)..), bias + relu, h2 in both layouts,
-        // partial head outputs of the tile's 32 columns
-        mbar_wait(tc_bar + 8u * 9u, tc_tiles & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+        // ---- epilogue: accumulator image in shared memory, then thread = one row of 16 columns (warp w: rows 32 (w & 3)..,
+        // columns 16 (w >> 2)..): bias + relu, h2 in both layouts, partial head outputs of the tile's 32 columns
+        jbwg::wait<0>();
+        jbwg::fence_acc(acc);
+        __syncthreads();                                          // both warpgroups' products retired: tcs overlays A slot 1
+        jbwg::store_acc_n32(acc, tcs, TC_LD);
+        __syncthreads();
         {
           const int q = warp & 3, cb = (warp >> 2) * 16, row = m0 + q * 32 + lane;
-          unsigned rr[16];
-          const unsigned taddr = tc_tmem + ((unsigned)(q * 32) << 16) + (unsigned)cb;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-              : "=r"(rr[0]), "=r"(rr[1]), "=r"(rr[2]), "=r"(rr[3]), "=r"(rr[4]), "=r"(rr[5]), "=r"(rr[6]), "=r"(rr[7]), "=r"(rr[8]),
-                "=r"(rr[9]), "=r"(rr[10]), "=r"(rr[11]), "=r"(rr[12]), "=r"(rr[13]), "=r"(rr[14]), "=r"(rr[15])
-              : "r"(taddr)
-              : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+          float rr[16];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float4 t = *reinterpret_cast<const float4*>(&tcs[(q * 32 + lane) * TC_LD + cb + 4 * c]);
+            rr[4 * c] = t.x; rr[4 * c + 1] = t.y; rr[4 * c + 2] = t.z; rr[4 * c + 3] = t.w;
+          }
           float v[16];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaxf(__uint_as_float(rr[i]) + PS[MAXO * PK + n0 + cb + i], 0.f);
+          for (int i = 0; i < 16; ++i) v[i] = fmaxf(rr[i] + PS[MAXO * PK + n0 + cb + i], 0.f);
           float4* o2 = reinterpret_cast<float4*>(a.h2 + (size_t)row * H + n0 + cb);
           float4* o2t = reinterpret_cast<float4*>(a.h2t + ((size_t)nt * B + row) * 32 + cb);
 #pragma unroll
@@ -741,7 +701,6 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             *reinterpret_cast<float4*>(sc) = make_float4(ph[0], ph[1], ph[2], ph[3]);
             *reinterpret_cast<float4*>(sc + 4) = make_float4(ph[4], ph[5], ph[6], ph[7]);
           }
-          asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
           __syncthreads();
           if (warp < 4) {
             const float4 u0 = *reinterpret_cast<const float4*>(sc), u1 = *reinterpret_cast<const float4*>(sc + 4);
@@ -751,8 +710,8 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           }
           __syncthreads();
         }
+        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // scratch reads above before later bulk copies / wgmma
         tc_g += (unsigned long long)NKC;
-        tc_tiles += 1u;
         TR(4);
       }
     } else
@@ -799,7 +758,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             }
           };
           if constexpr (ND <= 4) {                 // D <= 4 (CartPole): the input features unrolled, their 16 shared-memory loads in
-#pragma unroll                                     // flight together (the rolled loop exposed one load latency per feature: 3.3 us per panel)
+#pragma unroll                                     // flight together (the rolled loop exposed one load latency per feature)
             for (int i = 0; i < ND; ++i) if (i < D) feature(i);
           } else {
 #pragma unroll 1
@@ -868,7 +827,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     // tensor-core dh1 job: the first two W2^T chunks do not depend on the row phase, fetch them under it
     auto jb_issue_a = [&](int kt4, int nc, unsigned long long g) {
       const unsigned slot = (unsigned)(g % TC_NA);
-      const unsigned bar = tc_bar + 8u * (13u + slot), dst = tc_base + slot * TC_A_BYTES;
+      const unsigned bar = tc_bar + 8u * (TC_BAR_JB + slot), dst = tc_base + slot * TC_A_BYTES;
       mbar_expect_tx(bar, TC_A_BYTES);
       const float* src = a.W2Timg + ((size_t)kt4 * (H >> 5) + nc) * 4096;
       bulk_g2s(dst, src, 16384u, bar);
@@ -947,7 +906,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         // rank's gradient buffer, which the backward jobs below overwrite.
         const unsigned int target = a.xbase + (unsigned int)s + 1u;
         // message = two 8-byte words {row sum | tag}: an aligned 64-bit store is single-copy atomic, so payload and tag need
-        // no fence between them (a release-signalled message cost ~4 us per step); that the peer no longer READS this rank's
+        // no fence between them (a release-signalled message cost microseconds per step); that the peer no longer READS this rank's
         // gradient follows from program order on the peer (its loads of step s-1 returned before it got here)
         unsigned long long m1 = 0ull, m2 = 0ull;
         if (tid < a.world && tid != a.rank) {
@@ -1017,7 +976,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       if (TC && job < nJB) {
         // ---- tensor-core dh1 job: D[128 hidden units k][32 rows m] = sum_n W2[n][k] dh2[m][n]  (dh1 transposed) ---------
         // A chunk = hi | lo image of W2^T [128 k][32 n] (two 16 KB bulk copies, two chunks ahead); B chunk = dh2^T
-        // [32 m][32 n] = ((dout Wh) * relu'(h2)) generated by the threads, ONE float4 each; 4 x 3 tcgen05.mma per chunk.
+        // [32 m][32 n] = ((dout Wh) * relu'(h2)) generated by the threads, ONE float4 each; 4 x 3 wgmma per chunk and warpgroup.
         // Epilogue: mask by relu'(h1) (h1 recomputed from x: D FMAs), partial dW1 / db1 of this 32-row tile.
         const int kt4 = job / MT, mt = job - kt4 * MT, m0 = mt * 32, kin0 = kt4 * 128, NKC = H >> 5;
         if (job != cta && tid == 0) {
@@ -1028,10 +987,10 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         const int ml = tid >> 3, c8 = tid & 7;                      // this thread's element group: row m0 + ml, columns 4 c8 .. + 3 of a chunk
         const float* drow = &dsm[(m0 + ml) * MAXO];
         float4 hq = ldcg4(a.h2 + (size_t)(m0 + ml) * H + 4 * c8);     // h2 of chunk 0 (prefetched one chunk ahead below)
+        float acc[16];
         for (int nc = 0; nc < NKC; ++nc) {
           const unsigned long long g = jb_g + nc;
-          const unsigned slot = (unsigned)(g % TC_NA);
-          if (g >= TC_NA) mbar_wait(tc_bar + 8u * (10u + slot), (unsigned)((g / TC_NA - 1) & 1));     // chunk g - 3 retired: B slot free
+          const unsigned slot = (unsigned)(g % TC_NA);                 // B slot of chunk g - 3: retired (wait below)
           float4 wr[MAXO];
 #pragma unroll
           for (int o = 0; o < MAXO; ++o) wr[o] = o < nout ? *reinterpret_cast<const float4*>(&PS[o * PK + nc * 32 + 4 * c8]) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1039,45 +998,34 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           if (nc + 1 < NKC) hq = ldcg4(a.h2 + (size_t)(m0 + ml) * H + (nc + 1) * 32 + 4 * c8);
           const float4 dv = dh2_quad(drow, wr, hcur);
           const float4 lo = make_float4(tf32_lo(dv.x), tf32_lo(dv.y), tf32_lo(dv.z), tf32_lo(dv.w));
-          const unsigned bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES, off = tc_tile_off(ml, c8);
+          const unsigned bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES, off = tile_off(ml, c8);
           asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(bbuf + off), "f"(dv.x), "f"(dv.y), "f"(dv.z), "f"(dv.w) : "memory");
           asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(bbuf + 4096u + off), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
+          jbwg::wait<0>();                                              // chunk g - 1's products of this warpgroup retired
+          jbwg::fence_acc(acc);
           asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-          __syncthreads();
-          if (tid == 0) {
-            mbar_wait(tc_bar + 8u * (13u + slot), (unsigned)((g / TC_NA) & 1));               // W2^T chunk landed
-            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-            const unsigned abuf = tc_base + slot * TC_A_BYTES;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const unsigned ko = 32u * j;
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + ko), TC_IDESC_N32, (nc > 0 || j > 0) ? 1u : 0u);
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + 4096u + ko), TC_IDESC_N32, 1u);
-              tc_mma(tc_tmem, tc_desc(abuf + 16384u + ko), tc_desc(bbuf + ko), TC_IDESC_N32, 1u);
-            }
-            tc_commit(tc_bar + 8u * (10u + slot));
-            if (nc == NKC - 1) tc_commit(tc_bar + 8u * 9u);
-            if (nc + 2 < NKC) {                      // A ring: chunk nc + 2 goes where chunk nc - 1 lived
-              if (nc >= 1) mbar_wait(tc_bar + 8u * (10u + (unsigned)((g - 1) % TC_NA)), (unsigned)(((g - 1) / TC_NA) & 1));
-              jb_issue_a(kt4, nc + 2, g + 2);
-            }
-          }
+          __syncthreads();                                              // ... and those of the other warpgroup
+          if (tid == 0 && nc + 2 < NKC) jb_issue_a(kt4, nc + 2, g + 2);  // A ring: chunk nc + 2 goes where chunk nc - 1 lived
+          mbar_wait(tc_bar + 8u * (TC_BAR_JB + slot), (unsigned)((g / TC_NA) & 1));   // W2^T chunk landed
+          const unsigned aw = tc_base + slot * TC_A_BYTES + (unsigned)wg * 8192u;
+          jbwg::fence();
+          jbwg::mma3_n32(acc, aw, aw + 16384u, bbuf, bbuf + 4096u, nc == 0);
+          jbwg::commit();
         }
-        mbar_wait(tc_bar + 8u * 9u, tc_tiles & 1u);                 // (the "tile accumulated" barrier is shared with the forward phase)
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+        jbwg::wait<0>();
+        jbwg::fence_acc(acc);
+        __syncthreads();                                          // both warpgroups' products retired: tcs overlays A slot 1
+        jbwg::store_acc_n32(acc, tcs, TC_LD);
         __syncthreads();
         if (prefetchable(next)) { issue_stage(next); pre_job = next; }   // every MMA that read the rings has retired
         {
           const int q = warp & 3, cb = (warp >> 2) * 16, kin = kin0 + q * 32 + lane;
-          unsigned rr[16];
-          const unsigned taddr = tc_tmem + ((unsigned)(q * 32) << 16) + (unsigned)cb;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-              : "=r"(rr[0]), "=r"(rr[1]), "=r"(rr[2]), "=r"(rr[3]), "=r"(rr[4]), "=r"(rr[5]), "=r"(rr[6]), "=r"(rr[7]), "=r"(rr[8]),
-                "=r"(rr[9]), "=r"(rr[10]), "=r"(rr[11]), "=r"(rr[12]), "=r"(rr[13]), "=r"(rr[14]), "=r"(rr[15])
-              : "r"(taddr)
-              : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+          float rr[16];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float4 t = *reinterpret_cast<const float4*>(&tcs[(q * 32 + lane) * TC_LD + cb + 4 * c]);
+            rr[4 * c] = t.x; rr[4 * c + 1] = t.y; rr[4 * c + 2] = t.z; rr[4 * c + 3] = t.w;
+          }
           // h1[m][kin] > 0 ?  (same arithmetic as the forward phase: fma chain over the inputs, then + b1)
           float w1r[ND];
 #pragma unroll
@@ -1092,7 +1040,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             float h = 0.f;
 #pragma unroll
             for (int i = 0; i < ND; ++i) if (i < D) h = fmaf(xs[i * 32 + ml2], w1r[i], h);
-            const float dvv = (h + b1v > 0.f) ? __uint_as_float(rr[j]) : 0.f;
+            const float dvv = (h + b1v > 0.f) ? rr[j] : 0.f;
 #pragma unroll
             for (int i = 0; i < ND; ++i) if (i < D) wacc[i] = fmaf(dvv, xs[i * 32 + ml2], wacc[i]);
             wacc[ND] += dvv;
@@ -1102,7 +1050,6 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
 #pragma unroll
             for (int i = 0; i <= ND; ++i) if (i < D || i == ND) sc[i < D ? i : MAXD] = wacc[i];
           }
-          asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
           __syncthreads();
           if (warp < 4) {
             float* dstw = a.w1p + ((size_t)mt * H + kin) * (D + 1);
@@ -1113,8 +1060,8 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           __syncthreads();
         }
         if (tid < 4) asm volatile("red.release.gpu.global.add.u32 [%0], 1;\n" ::"l"(a.barrier + CTR_JB + kt4 * 4 + tid) : "memory");
+        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // scratch reads above before later bulk copies / wgmma
         jb_g += (unsigned long long)NKC;
-        tc_tiles += 1u;
         TR(16);
       } else if (!TC && job < nJB) {
         // ---- dh1 tile = ((dout Wh) * relu'(h2)) W2, masked by relu'(h1); partial dW1 / db1 ---------------
@@ -1204,11 +1151,11 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
 #pragma unroll
         for (int q = 0; q < 4; ++q) hq[q] = ldcg(h2col + (size_t)(4 * c8 + q) * 32);
         float b2acc = 0.f;
+        float acc[16];
         __syncthreads();                                            // xall complete
         for (int mc = 0; mc < NMC; ++mc) {
           const unsigned long long g = ja_g + mc;
-          const unsigned slot = (unsigned)(g % TC_NA);
-          if (g >= TC_NA) mbar_wait(tc_bar + 8u * (16u + slot), (unsigned)((g / TC_NA - 1) & 1));     // chunk g - 3 retired
+          const unsigned slot = (unsigned)(g % TC_NA);              // slots of chunk g - 3: retired (wait below)
           const unsigned abuf = tc_base + slot * TC_A_BYTES, bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES;
           // A chunk
           float hv[16];
@@ -1227,7 +1174,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           }
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
-            const unsigned off = tc_tile_off(r, half * 4 + c);
+            const unsigned off = tile_off(r, half * 4 + c);
             const float4 hi = make_float4(fmaxf(hv[4 * c] + b1v, 0.f), fmaxf(hv[4 * c + 1] + b1v, 0.f), fmaxf(hv[4 * c + 2] + b1v, 0.f), fmaxf(hv[4 * c + 3] + b1v, 0.f));
             const float4 lo = make_float4(tf32_lo(hi.x), tf32_lo(hi.y), tf32_lo(hi.z), tf32_lo(hi.w));
             asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(abuf + off), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
@@ -1253,41 +1200,35 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
               dv[q] = hc[q] > 0.f ? t : 0.f;                        // same arithmetic as dh2_quad
             }
             b2acc += (dv[0] + dv[1]) + (dv[2] + dv[3]);
-            const unsigned off = tc_tile_off(nl, c8);
+            const unsigned off = tile_off(nl, c8);
             asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(bbuf + off), "f"(dv[0]), "f"(dv[1]), "f"(dv[2]), "f"(dv[3]) : "memory");
             asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(bbuf + 4096u + off), "f"(tf32_lo(dv[0])), "f"(tf32_lo(dv[1])), "f"(tf32_lo(dv[2])), "f"(tf32_lo(dv[3])) : "memory");
           }
+          jbwg::wait<0>();                                          // chunk g - 1's products of this warpgroup retired
+          jbwg::fence_acc(acc);
           asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-          __syncthreads();
-          if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const unsigned ko = 32u * jj;
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + ko), TC_IDESC_N32, (mc > 0 || jj > 0) ? 1u : 0u);
-              tc_mma(tc_tmem, tc_desc(abuf + ko), tc_desc(bbuf + 4096u + ko), TC_IDESC_N32, 1u);
-              tc_mma(tc_tmem, tc_desc(abuf + 16384u + ko), tc_desc(bbuf + ko), TC_IDESC_N32, 1u);
-            }
-            tc_commit(tc_bar + 8u * (16u + slot));
-            if (mc == NMC - 1) tc_commit(tc_bar + 8u * 9u);
-          }
+          __syncthreads();                                          // ... and those of the other warpgroup
+          const unsigned aw = abuf + (unsigned)wg * 8192u;
+          jbwg::fence();
+          jbwg::mma3_n32(acc, aw, aw + 16384u, bbuf, bbuf + 4096u, mc == 0);
+          jbwg::commit();
         }
-        mbar_wait(tc_bar + 8u * 9u, tc_tiles & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+        jbwg::wait<0>();
+        jbwg::fence_acc(acc);
+        __syncthreads();                                          // both warpgroups' products retired: tcs overlays A slot 1
+        jbwg::store_acc_n32(acc, tcs, TC_LD);
+        __syncthreads();
         {
           const int q = warp & 3, cb = (warp >> 2) * 16, kk = k0 + q * 32 + lane;
-          unsigned rr[16];
-          const unsigned taddr = tc_tmem + ((unsigned)(q * 32) << 16) + (unsigned)cb;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-              : "=r"(rr[0]), "=r"(rr[1]), "=r"(rr[2]), "=r"(rr[3]), "=r"(rr[4]), "=r"(rr[5]), "=r"(rr[6]), "=r"(rr[7]), "=r"(rr[8]),
-                "=r"(rr[9]), "=r"(rr[10]), "=r"(rr[11]), "=r"(rr[12]), "=r"(rr[13]), "=r"(rr[14]), "=r"(rr[15])
-              : "r"(taddr)
-              : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+          float rr[16];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float4 t = *reinterpret_cast<const float4*>(&tcs[(q * 32 + lane) * TC_LD + cb + 4 * c]);
+            rr[4 * c] = t.x; rr[4 * c + 1] = t.y; rr[4 * c + 2] = t.z; rr[4 * c + 3] = t.w;
+          }
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
-            const float v = __uint_as_float(rr[i]);
+            const float v = rr[i];
             a.gW2[(size_t)(n0 + cb + i) * H + kk] = v;              // lanes = consecutive k: 128-byte rows
             sq = fmaf(v, v, sq);
           }
@@ -1296,11 +1237,10 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             t += __shfl_xor_sync(0xffffffffu, t, 1); t += __shfl_xor_sync(0xffffffffu, t, 2); t += __shfl_xor_sync(0xffffffffu, t, 4);
             if (c8 == 0) { a.gb2[n0 + nl] = t; sq = fmaf(t, t, sq); }
           }
-          asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
+          asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
           __syncthreads();
         }
         ja_g += (unsigned long long)NMC;
-        tc_tiles += 1u;
         TR(21);
       } else if (!TC && job < nJB + nJA) {
         // ---- a pair of dW2 tiles [n0.., k0..] = sum_m dh2[m, n] h1[m, k] sharing the dh2 panel; db2 = its row sums
@@ -1610,17 +1550,12 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     TR(27);
   }
   if (cta == 0 && tid == 0) { *a.step = step0 + a.n_steps; *a.cursor = cursor0 + a.n_steps; }
-  if (TC) {
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tc_tmem), "r"(32u) : "memory");
-  }
 }
 
 static int dsm_floats_for(int B) { return B * MAXO; }
 static size_t fused_smem(int B) { return sizeof(float) * (size_t)(SMALL_FLOATS + dsm_floats_for(B) + 2 * RED_FLOATS + R2_FLOATS + PS_FLOATS); }
 
-// Largest grid the cooperative launch can keep co-resident (one CTA per SM on B200) for minibatch size B.
+// Largest grid the cooperative launch can keep co-resident (one CTA per SM) for minibatch size B.
 static const void* fused_fn(bool tc, int A, int D) {
   const int na = A <= 2 ? 0 : (A <= 4 ? 1 : 2), nd = D <= 4 ? 0 : 1;
   static const void* const tab[4][3] = {
@@ -1662,9 +1597,9 @@ JB_API int jb_ppo_fused_run(const void* host_args, void* stream) {
   if (a.B <= 0 || a.B % 32 || a.B > MAX_B || a.H <= 0 || a.H % 32 || a.H > PK || a.D <= 0 || a.D > MAXD || a.nout <= 0 ||
       a.nout > MAXO || a.A <= 0 || a.A > jbppo::MAX_A || a.n_steps <= 0 || a.P4 <= 0)
     return JB_ERR_INVALID;
-  // Tensor-core instantiation (3xTF32 tcgen05 for the three dense products): needs 128-row tiles (B % 128 == 0,
-  // H % 128 == 0) and the W2 image workspaces.  It is parity-green but, as measured in round 2, SLOWER than the FFMA tiles
-  // at the reference minibatch (DESIGN.md 3b: with 128-row UMMA tiles only 32-64 CTAs work and each regenerates a 4x
+  // Tensor-core instantiation (3xTF32 wgmma for the three dense products): needs 128-row tiles (B % 128 == 0,
+  // H % 128 == 0) and the W2 image workspaces.  It is parity-green but SLOWER than the FFMA tiles at the reference
+  // minibatch (measured on H100 in DESIGN.md 8; the reason in DESIGN.md 3b: with 128-row tensor-core tiles only 32-64 CTAs work and each regenerates a 4x
   // larger operand panel on the CUDA cores, which is instruction-issue bound), so it is opt-in: JB_FUSED_TC=1.
   bool tc = false;
   if (const char* e = getenv("JB_FUSED_TC")) tc = atoi(e) != 0;

@@ -1,87 +1,35 @@
-// Large-M dense forward on the 5th-generation tensor cores (tcgen05 + TMEM), fp32-grade accuracy by
-// 3xTF32 operand splitting:  y[M,N] = act(x[M,K] W[N,K]^T + b).
+// Large-M dense forward on the Hopper tensor cores (wgmma), fp32-grade accuracy by 3xTF32 operand splitting:
+// y[M,N] = act(x[M,K] W[N,K]^T + b).
 //
 // Used for the products whose M is the number of env rows (act() over thousands of batched envs,
 // the PPO pre-pass over N*T rows: policy_value.py:19-22 / q_network.py:17-20 second layer), where a
-// 128x128 tile grid fills the 148 SMs.  The minibatch-sized products stay on the fp32 FFMA kernels
+// 128x128 tile grid fills the 132 SMs.  The minibatch-sized products stay on the fp32 FFMA kernels
 // (tile granularity M=128 would leave most SMs idle there, see DESIGN.md 4).
 //
-// Accuracy: tcgen05 kind::tf32 reads fp32 words from shared memory and keeps 10 mantissa bits.  Each
-// operand is split a = a_hi + a_lo with a_hi = the tf32 truncation the hardware applies to the raw fp32
-// word and a_lo = a - a_hi (computed here, itself fed as tf32), and three MMAs are accumulated in the
-// fp32 TMEM accumulator: a_hi b_hi + a_hi b_lo + a_lo b_hi.  Dropped term a_lo b_lo ~ 2^-22 relative:
-// the result matches the FFMA kernel to ~1e-6 (tests/test_tc_gemm_gpu.py), at 1/3 of the TF32 rate.
+// Accuracy: wgmma .tf32 reads fp32 words from shared memory and keeps 10 mantissa bits.  Each operand is
+// split a = a_hi + a_lo with a_hi = the tf32 truncation the hardware applies to the raw fp32 word and
+// a_lo = a - a_hi (computed here, itself fed as tf32), and three MMAs are accumulated in fp32 registers:
+// a_hi b_hi + a_hi b_lo + a_lo b_hi.  Dropped term a_lo b_lo ~ 2^-22 relative: the result matches the FFMA
+// kernel to ~1e-6 (tests/test_tc_gemm_gpu.py), at 1/3 of the TF32 rate.
 //
-// Structure (one CTA = one 128x128 output tile, 256 threads):
-//   * operands staged with cp.async (16-byte chunks) straight into the UMMA canonical K-major
-//     SWIZZLE_128B layout (128-byte rows, 1 KB 8-row atoms, chunk index XOR row) - coalesced global
-//     reads and conflict-free shared-memory writes; the lo tiles are derived in place by the loading threads;
-//   * one elected thread issues tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=128, K=8) x 4 k-steps x 3
-//     per 32-deep stage, accumulating in 128 TMEM columns; tcgen05.commit -> mbarrier frees the stage
-//     (3-stage ring, prefetch distance 2: loads of tiles kt+1, kt+2 overlap the tensor-core work on kt);
-//   * epilogue: tcgen05.ld 32x32b.x32 (each warp its own 32-lane TMEM quarter) -> bias/ReLU -> float4 stores.
-#include <cstdlib>
+// Structure (one CTA = one 128x128 output tile, 256 threads = two warpgroups of 64 output rows each):
+//   * operands staged with cp.async (16-byte chunks) straight into the canonical K-major SWIZZLE_128B
+//     layout (128-byte rows, 1 KB 8-row atoms, chunk index XOR row) - coalesced global reads and
+//     conflict-free shared-memory writes; the lo tiles are derived in place by the loading threads;
+//   * each warpgroup issues wgmma.m64n128k8.tf32 x 4 k-steps x 3 per 32-deep stage and leaves them in
+//     flight while the next stage's lo tiles are derived (3-stage ring, prefetch distance 2);
+//   * epilogue: bias/ReLU on the register accumulator -> float2 stores (four lanes = one 32-byte sector).
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 32, STAGES = 3, THREADS = 256;
 constexpr int TILE_BYTES = BM * BK * 4;                 // 16 KB per operand tile (hi or lo)
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;             // A_hi, A_lo, B_hi, B_lo
-constexpr int SBO = 1024;                               // bytes between consecutive 8-row swizzle atoms
-constexpr int TMEM_COLS = 128;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// K-major SWIZZLE_128B canonical layout: one 128-byte row per tile row (BK = 32 floats), eight rows per
-// 1 KB atom, 16-byte chunk index XOR-ed with the row index inside the atom (Swizzle<3,4,3>).  A row's eight
-// chunks stay inside one 128-byte line, so the cp.async stage fill is conflict-free AND coalesced.
-__device__ __forceinline__ uint32_t tile_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B (cute/arch/mma_sm100_desc.hpp bit layout).  `smem_addr` =
-// 1 KB-aligned tile base + 32 bytes per K=8 step inside the 128-byte swizzle atom.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, int variant = 0) {
-  (void)variant;
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);           // start address        bits [0,14)
-  d |= (uint64_t)1 << 16;                               // leading byte offset  bits [16,30): unused for swizzled K-major
-  d |= (uint64_t)((SBO >> 4) & 0x3FFF) << 32;           // stride byte offset   bits [32,46): 1 KB between 8-row atoms
-  d |= (uint64_t)1 << 46;                               // version = 1 (sm_100)
-  d |= (uint64_t)2 << 61;                               // layout_type = SWIZZLE_128B
-  return d;
-}
-
-// instruction descriptor: D = F32, A = B = TF32, both K-major, N = 128, M = 128
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(IDESC), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra WAIT_DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "WAIT_DONE:\n\t"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
+using jbwg::tile_off;
 
 // round-to-nearest tf32 (the tensor core itself truncates): removes the one-sided bias of the lo term
 __device__ __forceinline__ float tf32_rn(float x) {
@@ -96,36 +44,20 @@ __device__ __forceinline__ void cp16(uint32_t smem_addr, const void* gmem) {
 
 __global__ void __launch_bounds__(THREADS, 1)
 tc_linear_fwd_kernel(const float* __restrict__ X, const float* __restrict__ W, const float* __restrict__ bias,
-                     float* __restrict__ Y, int M, int N, int K, int relu, int variant) {
+                     float* __restrict__ Y, int M, int N, int K, int relu) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);   // swizzle atoms need 1 KB alignment
-  __shared__ __align__(8) uint64_t bar_free[STAGES];     // stage's MMAs retired -> smem may be refilled
-  __shared__ __align__(8) uint64_t bar_done;             // all MMAs retired -> epilogue
-  __shared__ uint32_t s_tmem;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) mbar_init(&bar_free[s], 1);
-    mbar_init(&bar_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&s_tmem)), "r"((uint32_t)TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const uint32_t tmem_acc = s_tmem;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
   const int nk = K / BK;
   // stage fill: A_hi / B_hi by cp.async into the canonical layout (one commit group per k-tile)
   auto issue_load = [&](int j) {
-    const int s = j % STAGES;
-    uint8_t* st = smem + (size_t)s * STAGE_BYTES;
-    if (j >= STAGES) mbar_wait(&bar_free[s], ((j / STAGES) - 1) & 1);     // previous tenant's MMAs retired
+    uint8_t* st = smem + (size_t)(j % STAGES) * STAGE_BYTES;
     const int k0 = j * BK;
 #pragma unroll
     for (int r = 0; r < (BM * BK / 4) / THREADS; ++r) {
@@ -138,11 +70,10 @@ tc_linear_fwd_kernel(const float* __restrict__ X, const float* __restrict__ W, c
   issue_load(0);
   if (nk > 1) issue_load(1);
   for (int kt = 0; kt < nk; ++kt) {
-    const int s = kt % STAGES;
-    uint8_t* st = smem + (size_t)s * STAGE_BYTES;
+    uint8_t* st = smem + (size_t)(kt % STAGES) * STAGE_BYTES;
     if (kt + 1 < nk) asm volatile("cp.async.wait_group 1;\n" ::: "memory");   // this thread's chunks of tile kt landed
     else asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-    // ---- lo tiles: a - trunc_tf32(a), by the thread that loaded the chunk ----------------------------
+    // ---- lo tiles: a - trunc_tf32(a), by the thread that loaded the chunk (tile kt - 1's MMAs still run) -----
 #pragma unroll
     for (int r = 0; r < (BM * BK / 4) / THREADS; ++r) {
       const int e = tid + r * THREADS, row = e >> 3, c = e & 7;
@@ -158,66 +89,37 @@ tc_linear_fwd_kernel(const float* __restrict__ X, const float* __restrict__ W, c
         *reinterpret_cast<float4*>(st + op * 2 * TILE_BYTES + TILE_BYTES + off) = lo;
       }
     }
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");     // generic-proxy smem writes -> async proxy (UMMA)
+    jbwg::wait<0>();                                                   // tile kt - 1's MMAs of this warpgroup retired
+    jbwg::fence_acc(acc);
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");     // generic-proxy smem writes -> async proxy (wgmma)
     __syncthreads();
-    // ---- MMA issue: one thread, 4 k-steps of 8, three products each -----------------------------------
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      const uint32_t a_hi = smem_u32(st), a_lo = a_hi + TILE_BYTES, b_hi = a_hi + 2 * TILE_BYTES, b_lo = a_hi + 3 * TILE_BYTES;
+    if (kt + 2 < nk) issue_load(kt + 2);       // into tile kt - 1's stage, which no MMA reads any more
+    // ---- MMA issue: this warpgroup's 64 rows, 4 k-steps of 8, three products each ----------------------
+    const uint32_t a_hi = smem_u32(st) + (uint32_t)wg * (64 * 128), a_lo = a_hi + TILE_BYTES;
+    const uint32_t b_hi = smem_u32(st) + 2 * TILE_BYTES, b_lo = b_hi + TILE_BYTES;
+    jbwg::fence();
 #pragma unroll
-      for (int j = 0; j < BK / 8; ++j) {
-        const uint32_t ko = (uint32_t)j * 32u;                   // K = 8 tf32 = 32 bytes along the swizzled row
-        const int v = variant & 1;
-        mma_tf32(tmem_acc, make_desc(a_hi + ko, v), make_desc(b_hi + ko, v), (kt > 0 || j > 0) ? 1u : 0u);
-        if (!(variant & 2)) {                                   // variant bit 1: single TF32 product (debug)
-          mma_tf32(tmem_acc, make_desc(a_hi + ko, v), make_desc(b_lo + ko, v), 1u);
-          mma_tf32(tmem_acc, make_desc(a_lo + ko, v), make_desc(b_hi + ko, v), 1u);
-        }
-      }
-      umma_commit(&bar_free[s]);
-      if (kt == nk - 1) umma_commit(&bar_done);
+    for (int j = 0; j < BK / 8; ++j) {
+      const uint32_t ko = (uint32_t)j * 32u;                   // K = 8 tf32 = 32 bytes along the swizzled row
+      jbwg::mma_n128(acc, jbwg::desc(a_hi + ko), jbwg::desc(b_hi + ko), (kt > 0 || j > 0) ? 1 : 0);
+      jbwg::mma_n128(acc, jbwg::desc(a_hi + ko), jbwg::desc(b_lo + ko), 1);
+      jbwg::mma_n128(acc, jbwg::desc(a_lo + ko), jbwg::desc(b_hi + ko), 1);
     }
-    if (kt + 2 < nk) issue_load(kt + 2);       // prefetch distance 2: the tensor core works on kt while kt+1, kt+2 stream in
+    jbwg::commit();
   }
-  // ---- epilogue ---------------------------------------------------------------------------------------
-  mbar_wait(&bar_done, 0);
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  {
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int row = m0 + q * 32 + lane;
-    const int cbase = (warp >> 2) * 64;           // warps 0-3: columns 0..63, warps 4-7: 64..127
+  jbwg::wait<0>();
+  jbwg::fence_acc(acc);
+  // ---- epilogue: accumulator element (row, col) of the fragment layout in csrc/wgmma.cuh ------------------
+  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-    for (int cc = 0; cc < 64; cc += 32) {
-      uint32_t r[32];
-      const uint32_t taddr = tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(cbase + cc);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-            "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-            "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-            "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      float* dst = Y + (size_t)row * N + n0 + cbase + cc;
-#pragma unroll
-      for (int i = 0; i < 32; i += 4) {
-        float4 o;
-        o.x = __uint_as_float(r[i + 0]) + (bias ? bias[n0 + cbase + cc + i + 0] : 0.f);
-        o.y = __uint_as_float(r[i + 1]) + (bias ? bias[n0 + cbase + cc + i + 1] : 0.f);
-        o.z = __uint_as_float(r[i + 2]) + (bias ? bias[n0 + cbase + cc + i + 2] : 0.f);
-        o.w = __uint_as_float(r[i + 3]) + (bias ? bias[n0 + cbase + cc + i + 3] : 0.f);
-        if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-        *reinterpret_cast<float4*>(dst + i) = o;
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_acc), "r"((uint32_t)TMEM_COLS) : "memory");
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    const float b0 = bias ? bias[col] : 0.f, b1 = bias ? bias[col + 1] : 0.f;
+    float2 o0 = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b1);
+    float2 o1 = make_float2(acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
+    if (relu) { o0.x = fmaxf(o0.x, 0.f); o0.y = fmaxf(o0.y, 0.f); o1.x = fmaxf(o1.x, 0.f); o1.y = fmaxf(o1.y, 0.f); }
+    *reinterpret_cast<float2*>(Y + (size_t)row * N + col) = o0;
+    *reinterpret_cast<float2*>(Y + (size_t)(row + 8) * N + col) = o1;
   }
 }
 
@@ -234,8 +136,6 @@ JB_API int jb_linear_fwd_tc(const float* x, const float* w, const float* b, floa
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(tc_linear_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
   dim3 grid(out_f / BN, M / BM);
-  int variant = 0;
-  if (const char* e = getenv("JB_TC_VARIANT")) variant = atoi(e);
-  tc_linear_fwd_kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(x, w, b, y, M, out_f, in_f, relu, variant);
+  tc_linear_fwd_kernel<<<grid, THREADS, smem, (cudaStream_t)stream>>>(x, w, b, y, M, out_f, in_f, relu);
   return jb_check_launch();
 }

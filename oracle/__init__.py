@@ -18,7 +18,7 @@ Pinning status
     reference's own act() / interact_callback() / learn() with every random primitive replaced by an injected draw
     (tests/golden/make_golden_collect.py, make_golden_ac.py, make_golden_ac_act.py).
   * CartPole / Pendulum / MountainCar physics: gym==0.23.0 is a third-party dependency that is
-    NOT vendored under /root/reference and is not installed here (requirements.txt:2).  Its
+    NOT vendored in the reference and is not installed (requirements.txt:2).  Its
     published equations are restated in oracle/classic_control.py; the reference's own tests for
     the envs check shapes only (jorldy/test/core/env/test_gym_env.py:5-32).  PARITY UNPINNED for
     the physics constants; pinned only for JORLDY's wrapper semantics (reward override, shapes).

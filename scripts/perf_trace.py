@@ -27,8 +27,9 @@ names = {0: "step start", 1: "P1 h1 generated", 2: "P1 panel landed", 3: "P1 mma
          17: "JA staged", 18: "JA dh2 gen", 19: "JA mma(last)", 20: "JA reduce(last)", 21: "JA end",
          22: "P3 jobs end", 28: "P1 stash issued", 29: "P1 stash landed", 31: "row: head outputs", 32: "row: math done",
          33: "JB dW1 staged", 34: "JB dW1 stored", 35: "P1 shuffles done", 36: "row: perm issued", 23: "norm partial + p/m/v issued", 24: "bar3", 25: "P5 fold", 26: "P5 end", 27: "bar5"}
-ghz = 1.965
-for cta in [0, 60, 147]:
+ghz = 1.98                                  # H100 SXM boost clock (clock64 ticks -> us)
+n = int((tr[:, 0] > 0).sum())               # CTAs of the launch
+for cta in sorted({0, n // 2, n - 1}):
     t = tr[cta]
     print(f"--- CTA {cta}")
     order = sorted([i for i in names if t[i] > 0], key=lambda i: t[i])
@@ -38,5 +39,5 @@ for cta in [0, 60, 147]:
         prev = t[i]
 # barrier waits: arrival spread
 for a_, b_, nm in [(5, 6, "bar1"), (23, 24, "bar3"), (26, 27, "bar5")]:
-    arr = tr[:148, a_] - tr[:148, 0]; dep = tr[:148, b_] - tr[:148, 0]
+    arr = tr[:n, a_] - tr[:n, 0]; dep = tr[:n, b_] - tr[:n, 0]
     print(f"{nm}: arrive min {arr.min()/ghz/1000:.2f} max {arr.max()/ghz/1000:.2f} (cta {arr.argmax()}) | depart-arrive min {(dep - arr).min()/ghz/1000:.2f} us")

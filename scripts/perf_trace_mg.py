@@ -33,7 +33,7 @@ names = {0: "step start", 5: "P1 end", 6: "bar1", 31: "row: head outputs", 32: "
          16: "JB end", 21: "JA end", 22: "P3 jobs end", 23: "p/m/v issued", 24: "bar3", 41: "X: peers' gradients complete (F1)",
          42: "X: chunk averaged + stored to all ranks", 43: "X: chunk tag published", 44: "X: all chunks of all owners landed",
          25: "P5 fold", 26: "P5 end", 27: "bar5"}
-ghz = 1.965
+ghz = 1.98                                  # H100 SXM boost clock (clock64 ticks -> us)
 if rank == 0:
     for cta in [0, 60, 147]:
         t = tr[cta]

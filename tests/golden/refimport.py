@@ -1,20 +1,21 @@
-"""Imports the UNMODIFIED reference (read-only /root/reference/jorldy) from a writable copy.
+"""Imports the UNMODIFIED reference (an upstream JORLDY checkout's `jorldy/` directory, named by the JORLDY_REFERENCE
+environment variable) from a writable copy.
 
-Only used by make_golden.py in the build container; never at test/bench time on the GPU box
-(where /root/reference does not exist).  A copy is needed because the reference's registries
-write `_*_dict.txt` next to themselves at import (core/agent/__init__.py:24 etc.).
+Used by the golden-vector makers and by tests/test_checkpoint_reference.py, which skips without it; no other test or
+benchmark needs the reference.  A copy is needed because the reference's registries write `_*_dict.txt` next to
+themselves at import (core/agent/__init__.py:24 etc.).
 """
 import os
 import shutil
 import sys
 import tempfile
 
-REF_ROOT = "/root/reference/jorldy"
+REF_ROOT = os.environ.get("JORLDY_REFERENCE", "")
 
 
 def import_reference():
-    if not os.path.isdir(REF_ROOT):
-        raise RuntimeError("reference not present (golden vectors can only be minted in the build container)")
+    if not REF_ROOT or not os.path.isdir(REF_ROOT):
+        raise RuntimeError("reference not present: set JORLDY_REFERENCE to an upstream JORLDY checkout's jorldy/ directory")
     dst = os.path.join(tempfile.gettempdir(), "jorldy_ref_copy")
     if not os.path.isdir(dst):
         shutil.copytree(REF_ROOT, dst, ignore=shutil.ignore_patterns("mlagents", "__pycache__"))

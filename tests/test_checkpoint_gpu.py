@@ -1,6 +1,6 @@
 """Checkpoint format parity (jorldy/core/agent/dqn.py:184-199, reinforce.py:128-142): torch.save of
 {"network": state_dict, "optimizer": state_dict} at path/ckpt with the reference's state_dict keys, so the
-reference's --eval can load B200-trained weights and vice versa; sync_in / sync_out round trip."""
+reference's --eval can load GPU-trained weights and vice versa; sync_in / sync_out round trip."""
 import os
 
 import numpy as np

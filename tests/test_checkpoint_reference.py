@@ -1,8 +1,8 @@
-"""SURVEY.md §8f-1 (CPU, build container only): a checkpoint WRITTEN by a jorldy_b200 agent on a B200
-(tests/golden/ckpt/<agent>/ckpt, produced by scripts/make_ckpt_fixtures.py) is loaded by the UNMODIFIED reference
-agent class (`load`, dqn.py:193-199 / reinforce.py:138-142) and the reference network's eval-mode forward on the
-recorded input equals what the B200 agent computed (fp32 tolerance 2e-5) — i.e. the reference's --eval can run
-B200-trained weights.  Skipped where /root/reference is absent (the GPU box)."""
+"""SURVEY.md §8f-1 (CPU): a checkpoint WRITTEN by a jorldy_b200 agent on the GPU (tests/golden/ckpt/<agent>/ckpt,
+produced by scripts/make_ckpt_fixtures.py) is loaded by the UNMODIFIED reference agent class (`load`, dqn.py:193-199 /
+reinforce.py:138-142) and the reference network's eval-mode forward on the recorded input equals what the GPU agent
+computed (fp32 tolerance 2e-5) — i.e. the reference's --eval can run GPU-trained weights.  Needs an upstream JORLDY
+checkout (JORLDY_REFERENCE=<checkout>/jorldy, tests/golden/refimport.py); skipped without one."""
 import os
 
 import numpy as np
@@ -26,9 +26,9 @@ CASES = {
 
 @pytest.fixture(scope="module")
 def agent_mod():
-    if not os.path.isdir("/root/reference/jorldy"):
-        pytest.skip("reference not present (build container only)")
-    from refimport import import_reference
+    from refimport import REF_ROOT, import_reference
+    if not REF_ROOT or not os.path.isdir(REF_ROOT):
+        pytest.skip("reference not present (set JORLDY_REFERENCE to an upstream JORLDY checkout's jorldy/ directory)")
     return import_reference()[0]
 
 
@@ -59,7 +59,7 @@ def test_reference_loads_b200_checkpoint(agent_mod, tag):
             np.testing.assert_allclose(agent.network(x, False).numpy(), exp["logits"], rtol=2e-5, atol=2e-5)
         else:
             np.testing.assert_allclose(agent.network(x).numpy(), exp["q"], rtol=2e-5, atol=2e-6)
-    # the reference's greedy act() on the loaded weights picks the actions the B200 agent picked
+    # the reference's greedy act() on the loaded weights picks the actions the GPU agent picked
     act = agent.act(exp["state"], training=False)["action"]
     if act.dtype.kind == "f":
         np.testing.assert_allclose(act, exp["action_eval"], rtol=0, atol=2e-6)
@@ -79,7 +79,7 @@ AC_CASES = {
 
 @pytest.mark.parametrize("tag", list(AC_CASES))
 def test_reference_loads_b200_actor_critic_checkpoint(agent_mod, tag):
-    """ddpg.py:186-197 / td3.py:232-246 / sac.py:321-339 load() on a checkpoint written by the B200 agent after two learns."""
+    """ddpg.py:186-197 / td3.py:232-246 / sac.py:321-339 load() on a checkpoint written by the GPU agent after two learns."""
     d = os.path.join(CKPT, tag)
     if not os.path.exists(os.path.join(d, "ckpt")):
         pytest.skip(f"no checkpoint fixture for {tag}")

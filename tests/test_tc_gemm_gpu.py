@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM 3xTF32 forward (csrc/tc_gemm.cu) vs a float64 reference and vs the fp32 FFMA kernel.
+"""wgmma 3xTF32 forward (csrc/tc_gemm.cu) vs a float64 reference and vs the fp32 FFMA kernel.
 Tolerance: max |err| <= 1e-5 * max(1, K/512) * max|y| (fp32-grade: three TF32 products recover ~22 mantissa bits;
 the tensor core's fp32 accumulation error grows linearly with the contraction length: 4e-6 at K=512, 1.6e-5 at
 K=3136 — both far inside the 1e-4 learner tolerance)."""
