@@ -68,6 +68,20 @@ jb_replay_store(void* ring, const void* batch, const int64_t* pos, int n, long l
 JB_API int
 jb_replay_gather(const void* ring, const int64_t* idx, int n, long long row_bytes, void* batch, void* stream);
 
+/* Single-frame Atari replay (csrc/frame_ring.cu): each lane of n keeps a ring of frames_per_lane 84x84 uint8 frames
+ * (frames [n, F, 7056]) with the episode-first position of each (first [n, F] int64) and its push count (head [n]).
+ * A frame reference is (lane << 40) | absolute position; the [4,84,84] stack it names is rebuilt on gather.
+ * push: obs / next_obs [n,4,84,84], done f32 [n].  next_obs NULL: push obs[:,3] as episode-first frames (after a reset);
+ * otherwise push next_obs[:,3], emit state_ref / next_ref (may be NULL), then obs[:,3] where done && auto_reset.
+ * gather: stacks of state_refs[idx[i]] / next_refs[idx[i]] (idx NULL: i) into [B,4,84,84]; a reference whose frames
+ * were overwritten is zero-filled and sets *status = 1. */
+JB_API int jb_frame_push(uint8_t* frames, int64_t* first, int64_t* head, int64_t frames_per_lane, const uint8_t* obs,
+                         const uint8_t* next_obs, const float* done, int auto_reset, int64_t* state_ref, int64_t* next_ref,
+                         int n, void* stream);
+JB_API int jb_frame_gather(const uint8_t* frames, const int64_t* first, const int64_t* head, int64_t frames_per_lane,
+                           int n_lanes, const int64_t* state_refs, const int64_t* next_refs, const int64_t* idx, int B,
+                           uint8_t* state_out, uint8_t* next_out, int32_t* status, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * PER sum-tree — jorldy/core/buffer/per_buffer.py:19-101.  tree is f64[2*capacity-1].
  * ------------------------------------------------------------------------------------------- */

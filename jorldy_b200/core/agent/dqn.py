@@ -159,6 +159,7 @@ class DQN(BaseAgent):
         batch, _, _, _ = self._sample()
         self._learn_batch(batch)
         st = self._stats[:2].cpu().numpy()
+        self.memory.check_frames()
         return {"loss": float(st[0]), "epsilon": self.epsilon, "max_Q": float(st[1])}
 
     def update_target(self):
@@ -265,6 +266,7 @@ class PER(DQN):
     def _per_result(self, stats_per):
         st = self._stats[:2].cpu().numpy()
         sp = stats_per.cpu().numpy()
+        self.memory.check_frames()
         return float(st[0]), float(st[1]), float(sp[0]), float(sp[1])
 
     def learn(self):
@@ -337,6 +339,7 @@ class Noisy(DQN):
         batch, _, _, _ = self._sample()
         self._learn_batch(batch)
         st = self._stats[:2].cpu().numpy()
+        self.memory.check_frames()
         s1, s2 = self.network.get_sig_w_mean()
         return {"loss": float(st[0]), "max_Q": float(st[1]), "sig_w1": float(s1.item()), "sig_w2": float(s2.item())}
 
@@ -417,6 +420,7 @@ class C51(DQN, _Distributional):
         batch, _, _, _ = self._sample()
         self._dist_learn(batch, None, 0, [None, None, None])
         st = self._stats.cpu().numpy()
+        self.memory.check_frames()
         return {"loss": float(st[0]), "epsilon": self.epsilon, "max_Q": float(st[1]), "max_logit": float(st[2]),
                 "min_logit": float(st[3])}
 
@@ -463,6 +467,7 @@ class Rainbow(PER, _Distributional):
         self.memory.update_priorities(indices, prio)
         st = self._stats.cpu().numpy()
         sp = stats_per.cpu().numpy()
+        self.memory.check_frames()
         return {"loss": float(st[0]), "beta": self.beta, "max_Q": float(st[1]), "max_logit": float(st[2]),
                 "min_logit": float(st[3]), "sampled_p": float(sp[0]), "mean_p": float(sp[1])}
 

@@ -1,0 +1,132 @@
+"""Single-frame replay for Atari-shaped observations (csrc/frame_ring.cu).
+
+A replay slot of the duplicated layout holds `state` and `next_state` as two uint8 [4,84,84] stacks: 56,448 B, with every
+84x84 frame stored 8 times.  With a frame store attached, each batched env row (a lane) pushes every frame once into its
+own ring of `F` frames, and the replay's `state` / `next_state` fields hold int64 frame references (8 B each).
+`ReplayBuffer.gather_device` turns them back into the same [B,4,84,84] stacks, bit for bit, so sampling, learn() and the
+PER tree do not change.
+
+This module owns the format: the sizing of the rings, the reference encoding ((lane << 40) | absolute frame position),
+the push of one env step and the gather.  A reference whose frames have been overwritten is never returned silently:
+the gather kernel sets a status word and `check()` raises `FrameEvictedError`.
+"""
+import torch
+
+from ..dev import C, ptr, stream_ptr
+
+FRAME_BYTES = 84 * 84
+STACK = 4
+POS_BITS = 40
+FRAME_KEYS = ("state", "next_state")
+
+
+class FrameEvictedError(RuntimeError):
+    """A replay slot referenced a frame that its lane's ring had already overwritten."""
+
+
+def frames_per_lane(capacity, num_lanes, n_step, margin=None):
+    """Ring length F per lane for a replay of `capacity` slots filled by `num_lanes` lanes.
+
+    The ring holds ceil(C/N) transitions per lane, the n-step window emits a transition up to n_step env steps after its
+    state, and the oldest stack reaches 3 frames further back (+ 4).  Episode resets push one extra frame each; the
+    default margin of ceil(ceil(C/N)/16) frames covers a reset every 16 steps of every lane."""
+    per_lane = -(-int(capacity) // int(num_lanes))
+    if margin is None:
+        margin = -(-per_lane // 16)
+    return per_lane + int(n_step) + 4 + int(margin)
+
+
+def store_bytes(capacity, num_lanes, n_step, margin=None):
+    """HBM taken by the frame rings (the replay adds 16 B of references per slot)."""
+    return int(num_lanes) * frames_per_lane(capacity, num_lanes, n_step, margin) * FRAME_BYTES
+
+
+def check_refs(transitions):
+    """Raises ValueError unless every transition carries frame references (int64 [N]) under `state` / `next_state`."""
+    for t in transitions:
+        for k in FRAME_KEYS:
+            v = t.get(k)
+            if not (torch.is_tensor(v) and v.dtype == torch.int64 and v.dim() == 1):
+                shape = tuple(v.shape) if hasattr(v, "shape") else type(v).__name__
+                raise ValueError(
+                    f"this replay keeps '{k}' as single-frame references (a frame store was attached when the Atari "
+                    f"collector started), so it cannot store stacked observations (got {shape}); store them into a "
+                    f"replay that no collector has attached a frame store to")
+
+
+class FrameStore:
+    def __init__(self, num_lanes, frames_per_lane, device):
+        self.n, self.F = int(num_lanes), int(frames_per_lane)
+        if self.F < 8:
+            raise ValueError(f"frames_per_lane must be at least 8, got {self.F}")
+        if self.n >= 1 << (63 - POS_BITS):
+            raise ValueError(f"{self.n} lanes do not fit the frame reference encoding")
+        self.device = device
+        # only positions a push has written are ever read (the gather checks residency), so the frames start unset
+        self.frames = torch.empty((self.n, self.F, FRAME_BYTES), dtype=torch.uint8, device=device)
+        self.first = torch.zeros((self.n, self.F), dtype=torch.int64, device=device)
+        self.head = torch.zeros(self.n, dtype=torch.int64, device=device)
+        # written by the gather kernel only on an evicted reference; pinned host memory, so reading it after the
+        # stream synchronisation that learn() already does costs no copy
+        self.status = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+        self.started = False
+
+    @classmethod
+    def for_replay(cls, capacity, num_lanes, n_step, device, margin=None):
+        return cls(num_lanes, frames_per_lane(capacity, num_lanes, n_step, margin), device)
+
+    def start(self, obs):
+        """Pushes obs[:,3] of every lane as an episode-first frame (obs: the [N,4,84,84] stacks after a reset)."""
+        self._check_obs(obs)
+        C.jb_frame_push(ptr(self.frames), ptr(self.first), ptr(self.head), self.F, ptr(obs), 0, 0, 0, 0, 0, self.n,
+                        stream_ptr())
+        self.started = True
+
+    def push(self, obs, next_obs, done, auto_reset):
+        """One env step: next_obs[:,3] continues each lane's episode; where done and the env auto-reset, obs[:,3] starts
+        the next one.  Returns (state_ref, next_ref), int64 [N]: the stack acted on and the stack after the step."""
+        if not self.started:
+            raise RuntimeError("FrameStore.start() must push the reset observation first")
+        self._check_obs(obs)
+        self._check_obs(next_obs)
+        refs = torch.empty((2, self.n), dtype=torch.int64, device=self.device)
+        C.jb_frame_push(ptr(self.frames), ptr(self.first), ptr(self.head), self.F, ptr(obs), ptr(next_obs),
+                        ptr(done.contiguous()), int(bool(auto_reset)), ptr(refs[0]), ptr(refs[1]), self.n, stream_ptr())
+        return refs[0], refs[1]
+
+    def gather(self, state_refs, next_refs, idx=None):
+        """Stacks [B,4,84,84] of state_refs[idx] and next_refs[idx] (idx None: all of them).  An evicted reference
+        comes back zero-filled and makes the next check() raise."""
+        B = int(idx.shape[0]) if idx is not None else int(state_refs.shape[0])
+        state = torch.empty((B, STACK, 84, 84), dtype=torch.uint8, device=self.device)
+        nxt = torch.empty_like(state)
+        if B == 0:
+            return state, nxt
+        C.jb_frame_gather(ptr(self.frames), ptr(self.first), ptr(self.head), self.F, self.n, ptr(state_refs.contiguous()),
+                          ptr(next_refs.contiguous()), ptr(idx), B, ptr(state), ptr(nxt), ptr(self.status), stream_ptr())
+        return state, nxt
+
+    def check(self):
+        """Raises FrameEvictedError if a gather so far met a reference to an overwritten frame."""
+        torch.cuda.current_stream(self.device).synchronize()
+        if int(self.status[0]) != 0:
+            raise FrameEvictedError(
+                f"the replay sampled a frame that its lane's ring of {self.F} frames had already overwritten; the batch "
+                f"gathered with it is invalid (more episode resets than the ring's margin covers)")
+
+    def _check_obs(self, obs):
+        if obs.dtype != torch.uint8 or tuple(obs.shape) != (self.n, STACK, 84, 84) or not obs.is_contiguous():
+            raise ValueError(f"expected contiguous uint8 [{self.n},4,84,84] stacks, got {obs.dtype} {tuple(obs.shape)}")
+
+
+def attach(env, memory, n_step):
+    """Gives `memory` a frame store sized for `env`'s lanes when the env produces frame stacks (`env.frame_stack`) and
+    the memory is an empty replay ring; returns the store, or None (the memory keeps whole stacks)."""
+    from .replay_buffer import ReplayBuffer
+    if not getattr(env, "frame_stack", False) or not isinstance(memory, ReplayBuffer):
+        return None
+    if memory.fields is not None or memory.size > 0 or memory.frames is not None:
+        return None
+    store = FrameStore.for_replay(memory.buffer_size, env.num_envs, n_step, memory.device)
+    memory.frames = store
+    return store

@@ -10,11 +10,15 @@ dtypes in HBM: uint8 observations stay uint8 (the learner casts, base.py:61-73);
 are stored as float32 (the learner casts them to float32 anyway — same rounding, done once);
 bool -> uint8; int64 kept.  `sample()` returns numpy arrays with the dtypes the reference's
 `stack_transition` would have produced.
+
+Atari-shaped collectors attach a single-frame store (frame_store.py): `state` / `next_state` then hold int64 frame
+references, `gather_device` rebuilds the same uint8 stacks from them, and stacked stores are refused.
 """
 import numpy as np
 import torch
 
 from ..dev import C, ptr, require_cuda, stream_ptr
+from . import frame_store
 from .base import BaseBuffer
 
 _STORE_DTYPE = {np.dtype("float64"): torch.float32, np.dtype("float32"): torch.float32,
@@ -35,6 +39,7 @@ class ReplayBuffer(BaseBuffer):
         self.buffer_counter = 0
         self.fields = None          # key -> tensor | list[tensor]
         self._np_dtype = {}         # key / (key, i) -> numpy dtype the reference would return
+        self.frames = None          # FrameStore (frame_store.py): `state` / `next_state` then hold frame references
 
     # ---- storage ------------------------------------------------------------------------------
     def _alloc_one(self, tag, sample):
@@ -71,6 +76,8 @@ class ReplayBuffer(BaseBuffer):
 
     def _write(self, transitions):
         """Writes the stacked transitions into the ring; returns the number of rows written."""
+        if self.frames is not None:
+            frame_store.check_refs(transitions)
         if self.fields is None:
             self._allocate(transitions[0])
         n = sum(int(np.shape(t["reward"])[0]) if "reward" in t else 1 for t in transitions)
@@ -122,9 +129,20 @@ class ReplayBuffer(BaseBuffer):
         """idx: int64 device tensor of ring positions -> dict of device tensors (stored dtypes)."""
         out = {}
         idx = idx.to(torch.int64).contiguous()
+        stacks = {}
+        if self.frames is not None:
+            stacks = dict(zip(frame_store.FRAME_KEYS, self.frames.gather(self.fields["state"], self.fields["next_state"], idx)))
         for key, src in self.fields.items():
-            out[key] = [self._gather(s, idx) for s in src] if isinstance(src, list) else self._gather(src, idx)
+            if key in stacks:
+                out[key] = stacks[key]
+            else:
+                out[key] = [self._gather(s, idx) for s in src] if isinstance(src, list) else self._gather(src, idx)
         return out
+
+    def check_frames(self):
+        """Raises if a gather so far handed out an evicted frame (no-op without a frame store).  Synchronises the stream."""
+        if self.frames is not None:
+            self.frames.check()
 
     def _to_numpy(self, dev_dict):
         out = {}
@@ -133,6 +151,7 @@ class ReplayBuffer(BaseBuffer):
                 out[key] = [self._cast_np(v.cpu().numpy(), self._np_dtype[(key, i)]) for i, v in enumerate(val)]
             else:
                 out[key] = self._cast_np(val.cpu().numpy(), self._np_dtype[key])
+        self.check_frames()
         return out
 
     @staticmethod

@@ -7,7 +7,7 @@ randomness).
 """
 import torch
 
-from .buffer import DeviceRollout
+from .buffer import DeviceRollout, frame_store
 
 
 class RolloutCollector:
@@ -116,16 +116,24 @@ class ReplayCollector:
         if apex:
             agent.set_actor_epsilons(env.num_envs, total=max(agent.num_workers, env.num_envs, 2))
         env.reset_device()
+        # Atari-shaped envs: every frame is pushed once and the replay stores frame references (buffer/frame_store.py)
+        self.frames = frame_store.attach(env, agent.memory, n)
+        if self.frames is not None:
+            self.frames.start(env.obs)
 
     def run_round(self, step):
         env, agent = self.env, self.agent
         batches = []
         for _ in range(self.update_period):
-            state = env.obs.clone()
+            state = env.obs if self.frames is not None else env.obs.clone()
             action, q_sel = agent.act_device(agent._net_input(state), True)
             next_obs, reward, done = env.step_device(action)
+            if self.frames is not None:
+                state, next_state = self.frames.push(env.obs, next_obs, done, env.auto_reset)
+            else:
+                next_state = next_obs.clone()
             tr = {"state": state, "action": action.view(action.shape[0], -1).clone(), "reward": reward.clone(), "done": done.clone(),
-                  "next_state": next_obs.clone()}
+                  "next_state": next_state}
             if self.assembler is not None:
                 if self.assembler.apex:
                     tr["q"] = q_sel.clone()

@@ -16,6 +16,10 @@ _ACTIONS = {"breakout": 4, "pong": 6, "asterix": 9, "assault": 7, "seaquest": 18
 
 class SyntheticAtari(BaseEnv):
     action_type = "discrete"
+    # frame-stack contract: obs / next_obs are [N,4,84,84] stacks whose slot 3 is the newest frame and slots 0..2 the
+    # previous stack's 1..3, and a reset stack is its first frame tiled x4, so a replay can store each frame once
+    # (buffer/frame_store.py)
+    frame_stack = True
 
     def __init__(self, name="breakout", num_envs=1, seed=0, id=0, device=None, auto_reset=None, img_width=84,
                  img_height=84, stack_frame=4, action_size=None, train_mode=True, **kwargs):
