@@ -216,11 +216,12 @@ JB_API int jb_noisy_grad(const float* dw_eff, const float* db_eff, const float* 
  * ------------------------------------------------------------------------------------------- */
 JB_API int jb_grad_partials_count(long long P);
 JB_API int jb_grad_sumsq(const float* g, long long P, float* partials, long long* step, void* stream);
-JB_API int jb_adam_step(float* p, const float* g, float* m, float* v, long long P, const float* lr, float beta1,
-                        float beta2, float eps, const long long* step, const float* partials, int n_partials,
+/* beta1, beta2 and alpha are doubles so that 1 - beta is formed before rounding to fp32, as torch does */
+JB_API int jb_adam_step(float* p, const float* g, float* m, float* v, long long P, const float* lr, double beta1,
+                        double beta2, float eps, const long long* step, const float* partials, int n_partials,
                         float max_norm, float* norm_out, void* stream);
 JB_API int jb_rmsprop_centered_step(float* p, const float* g, float* square_avg, float* grad_avg, long long P,
-                                    const float* lr, float alpha, float eps, const float* partials, int n_partials,
+                                    const float* lr, double alpha, float eps, const float* partials, int n_partials,
                                     float max_norm, float* norm_out, void* stream);
 JB_API int jb_copy_f32(float* dst, const float* src, long long P, void* stream);
 

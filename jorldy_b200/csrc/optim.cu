@@ -70,7 +70,9 @@ __device__ __forceinline__ float clip_coef_from_partials(const float* __restrict
   return s_coef;
 }
 
-struct AdamHP { float b1, b2, eps, max_norm; };
+// 1 - beta is rounded from the double value (as torch forms it), not computed from the rounded fp32 beta: for
+// beta2 = 0.999 the latter is off by 1.3e-5 relative.  The bias corrections use the double betas too.
+struct AdamHP { float b1, b2, one_m_b1, one_m_b2, eps, max_norm; double b1d, b2d; };
 
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
@@ -78,11 +80,11 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
             const float* __restrict__ partials, int n_partials, float* __restrict__ norm_out) {
   const float coef = clip_coef_from_partials(partials, n_partials, hp.max_norm, blockIdx.x == 0 ? norm_out : nullptr);
   const double t = (double)(*step_ptr);
-  const double bc1 = 1.0 - pow((double)hp.b1, t);
-  const double bc2 = 1.0 - pow((double)hp.b2, t);
+  const double bc1 = 1.0 - pow(hp.b1d, t);
+  const double bc2 = 1.0 - pow(hp.b2d, t);
   const float step_size = (float)((double)(*lr_ptr) / bc1);
   const float bc2_sqrt = (float)sqrt(bc2);
-  const float one_m_b1 = 1.f - hp.b1, one_m_b2 = 1.f - hp.b2;
+  const float one_m_b1 = hp.one_m_b1, one_m_b2 = hp.one_m_b2;
 
   auto upd = [&](float& pp, float gg, float& mm, float& vv) {
     gg *= coef;
@@ -108,7 +110,7 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
   }
 }
 
-struct RmsHP { float alpha, eps, max_norm; };
+struct RmsHP { float alpha, one_m_alpha, eps, max_norm; };
 
 __global__ void __launch_bounds__(256)
 rmsprop_centered_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq,
@@ -116,7 +118,7 @@ rmsprop_centered_kernel(float* __restrict__ p, const float* __restrict__ g, floa
                         const float* __restrict__ partials, int n_partials, float* __restrict__ norm_out) {
   const float coef = clip_coef_from_partials(partials, n_partials, hp.max_norm, blockIdx.x == 0 ? norm_out : nullptr);
   const float lr = *lr_ptr;
-  const float one_m_a = 1.f - hp.alpha;
+  const float one_m_a = hp.one_m_alpha;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < P; i += (long long)gridDim.x * blockDim.x) {
     const float gg = g[i] * coef;
     float s = sq[i], a = ga[i];
@@ -156,23 +158,24 @@ JB_API int jb_grad_sumsq(const float* g, long long P, float* partials, long long
 }
 
 // max_norm <= 0 disables clipping.  norm_out (device float, may be NULL) receives ||g||_2.
-JB_API int jb_adam_step(float* p, const float* g, float* m, float* v, long long P, const float* lr, float beta1,
-                        float beta2, float eps, const long long* step, const float* partials, int n_partials,
+JB_API int jb_adam_step(float* p, const float* g, float* m, float* v, long long P, const float* lr, double beta1,
+                        double beta2, float eps, const long long* step, const float* partials, int n_partials,
                         float max_norm, float* norm_out, void* stream) {
   if (!p || !g || !m || !v || !lr || !step || P <= 0) return JB_ERR_INVALID;
   if (max_norm > 0.f && (!partials || n_partials <= 0)) return JB_ERR_INVALID;
-  AdamHP hp{beta1, beta2, eps, partials ? max_norm : 0.f};
+  AdamHP hp{(float)beta1, (float)beta2, (float)(1.0 - beta1), (float)(1.0 - beta2), eps, partials ? max_norm : 0.f,
+            beta1, beta2};
   int blocks = jb_grid_for(P / 4 + 1, 256, 2);
   adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, P, lr, hp, step, partials, partials ? n_partials : 0, norm_out);
   return jb_check_launch();
 }
 
 JB_API int jb_rmsprop_centered_step(float* p, const float* g, float* square_avg, float* grad_avg, long long P,
-                                    const float* lr, float alpha, float eps, const float* partials, int n_partials,
+                                    const float* lr, double alpha, float eps, const float* partials, int n_partials,
                                     float max_norm, float* norm_out, void* stream) {
   if (!p || !g || !square_avg || !grad_avg || !lr || P <= 0) return JB_ERR_INVALID;
   if (max_norm > 0.f && (!partials || n_partials <= 0)) return JB_ERR_INVALID;
-  RmsHP hp{alpha, eps, partials ? max_norm : 0.f};
+  RmsHP hp{(float)alpha, (float)(1.0 - alpha), eps, partials ? max_norm : 0.f};
   int blocks = jb_grid_for(P, 256 * 4, 2);
   rmsprop_centered_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, g, square_avg, grad_avg, P, lr, hp, partials,
                                                                   partials ? n_partials : 0, norm_out);
