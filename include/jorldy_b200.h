@@ -81,6 +81,13 @@ JB_API int jb_frame_push(uint8_t* frames, int64_t* first, int64_t* head, int64_t
 JB_API int jb_frame_gather(const uint8_t* frames, const int64_t* first, const int64_t* head, int64_t frames_per_lane,
                            int n_lanes, const int64_t* state_refs, const int64_t* next_refs, const int64_t* idx, int B,
                            uint8_t* state_out, uint8_t* next_out, int32_t* status, void* stream);
+/* conv1's column matrix read straight from the ring (the CNN head's 4x84x84 input, 8x8 kernel, stride 4): col
+ * [M*20*20, 256] f32 = im2col of the stacks of refs[idx[i]] (idx int32, NULL: i), each value (float)v / 255.0f, so it is
+ * bit-equal to jb_frame_gather followed by jb_im2col_u8.  A non-resident reference writes zero rows and sets *status = 1.
+ * frames must be 4-byte and col 16-byte aligned. */
+JB_API int jb_im2col_u8_frames(const uint8_t* frames, const int64_t* first, const int64_t* head, int64_t frames_per_lane,
+                               int n_lanes, const int64_t* refs, const int32_t* idx, int M, float* col, int32_t* status,
+                               void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * PER sum-tree — jorldy/core/buffer/per_buffer.py:19-101.  tree is f64[2*capacity-1].

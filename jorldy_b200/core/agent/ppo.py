@@ -15,7 +15,7 @@ keys.  What changes is where the work happens:
 import numpy as np
 import torch
 
-from ..buffer import RolloutBuffer
+from ..buffer import FrameRollout, RolloutBuffer
 from ..dev import C, ptr, require_cuda, stream_ptr
 from ..network import Network
 from ..optimizer import Optimizer
@@ -309,11 +309,18 @@ class PPO(BaseAgent):
         return self._learn_tensors(hin["state"], hin["action"], hin["reward"], hin["done"], next_state=hin["next_state"])
 
     def learn_rollout(self, rollout):
-        """Resident path: `rollout` is a DeviceRollout filled by the batched collect loop."""
+        """Resident path: `rollout` is a DeviceRollout (or FrameRollout) filled by the batched collect loop."""
         N, T = rollout.N, rollout.T
-        res = self._learn_tensors(rollout.state.view(N * T, -1), rollout.action.view(N * T, -1) if self.continuous
+        frames = isinstance(rollout, FrameRollout)
+        if frames:          # the CNN head reads the states' stacks from the rollout's frame ring
+            state, last = rollout.rows(), rollout.last_rows()
+        else:
+            state, last = rollout.state.view(N * T, -1), rollout.last_next_state
+        res = self._learn_tensors(state, rollout.action.view(N * T, -1) if self.continuous
                                   else rollout.action.view(N * T), rollout.reward.view(N * T),
-                                  rollout.done.view(N * T), last_next_state=rollout.last_next_state)
+                                  rollout.done.view(N * T), last_next_state=last)
+        if frames:
+            rollout.frames.check()      # after _learn_tensors' device->host read: no further wait
         rollout.clear()
         return res
 

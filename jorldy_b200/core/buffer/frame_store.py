@@ -6,9 +6,12 @@ own ring of `F` frames, and the replay's `state` / `next_state` fields hold int6
 `ReplayBuffer.gather_device` turns them back into the same [B,4,84,84] stacks, bit for bit, so sampling, learn() and the
 PER tree do not change.
 
+PPO's frame rollout (`FrameRollout`) keeps its states on a frame store too: `frames_per_rollout(T)` sizes the ring, and
+`FrameRows` hands the CNN head a view of the referenced stacks whose conv1 im2col reads the ring directly.
+
 This module owns the format: the sizing of the rings, the reference encoding ((lane << 40) | absolute frame position),
-the push of one env step and the gather.  A reference whose frames have been overwritten is never returned silently:
-the gather kernel sets a status word and `check()` raises `FrameEvictedError`.
+the push of one env step, the gather and conv1's im2col.  A reference whose frames have been overwritten is never
+returned silently: the gather and im2col kernels set a status word and `check()` raises `FrameEvictedError`.
 """
 import torch
 
@@ -34,6 +37,17 @@ def frames_per_lane(capacity, num_lanes, n_step, margin=None):
     if margin is None:
         margin = -(-per_lane // 16)
     return per_lane + int(n_step) + 4 + int(margin)
+
+
+def frames_per_rollout(T):
+    """Ring length F per lane for an on-policy rollout of T steps: max(2T + 4, 8).
+
+    A rollout's first state is the newest frame pushed before it, at position h0 - 1 (h0: the lane's head when the
+    rollout starts), and its stack reaches back to h0 - 4.  Each of the T steps pushes at most 2 frames (the newest
+    frame, and the reset frame after an auto-reset), so when learn_rollout() reads the rollout the head is at most
+    h0 + 2T, and every frame the rollout references lies in [h0 - 4, h0 + 2T): 2T + 4 frames, whatever the dones.  The
+    next rollout's pushes start only after that read.  FrameStore (and jb_frame_push) need at least 8 frames."""
+    return max(2 * int(T) + 4, 8)
 
 
 def store_bytes(capacity, num_lanes, n_step, margin=None):
@@ -82,14 +96,17 @@ class FrameStore:
                         stream_ptr())
         self.started = True
 
-    def push(self, obs, next_obs, done, auto_reset):
+    def push(self, obs, next_obs, done, auto_reset, out=None):
         """One env step: next_obs[:,3] continues each lane's episode; where done and the env auto-reset, obs[:,3] starts
-        the next one.  Returns (state_ref, next_ref), int64 [N]: the stack acted on and the stack after the step."""
+        the next one.  Returns (state_ref, next_ref), int64 [N]: the stack acted on and the stack after the step, as
+        the rows of `out` (int64 [2, N], contiguous) when given."""
         if not self.started:
             raise RuntimeError("FrameStore.start() must push the reset observation first")
         self._check_obs(obs)
         self._check_obs(next_obs)
-        refs = torch.empty((2, self.n), dtype=torch.int64, device=self.device)
+        if out is not None and (out.dtype != torch.int64 or tuple(out.shape) != (2, self.n) or not out.is_contiguous()):
+            raise ValueError(f"expected a contiguous int64 [2,{self.n}] reference buffer, got {out.dtype} {tuple(out.shape)}")
+        refs = out if out is not None else torch.empty((2, self.n), dtype=torch.int64, device=self.device)
         C.jb_frame_push(ptr(self.frames), ptr(self.first), ptr(self.head), self.F, ptr(obs), ptr(next_obs),
                         ptr(done.contiguous()), int(bool(auto_reset)), ptr(refs[0]), ptr(refs[1]), self.n, stream_ptr())
         return refs[0], refs[1]
@@ -117,6 +134,37 @@ class FrameStore:
     def _check_obs(self, obs):
         if obs.dtype != torch.uint8 or tuple(obs.shape) != (self.n, STACK, 84, 84) or not obs.is_contiguous():
             raise ValueError(f"expected contiguous uint8 [{self.n},4,84,84] stacks, got {obs.dtype} {tuple(obs.shape)}")
+
+
+class FrameRows:
+    """The [M,4,84,84] stacks named by `refs` (int64 [M]) on `store`, as the CNN head's input: it has shape[0], row
+    slices (inference chunks) and `im2col`, which writes conv1's column matrix straight from the ring.  data_ptr() is
+    the refs tensor's, so a CUDA graph keyed on the input's pointer is replayed only over the same reference rows."""
+
+    def __init__(self, store, refs):
+        self.store, self.refs = store, refs
+
+    @property
+    def shape(self):
+        return (int(self.refs.shape[0]), STACK, 84, 84)
+
+    def __getitem__(self, rows):
+        if not isinstance(rows, slice):
+            raise TypeError("FrameRows supports row slices only")
+        return FrameRows(self.store, self.refs[rows])
+
+    def data_ptr(self):
+        return self.refs.data_ptr()
+
+    def im2col(self, idx, M, col):
+        """col [M*400, 256] f32 <- conv1's im2col of the stacks refs[idx[i]] (idx int32 [M], None: rows 0..M-1), bit-equal
+        to gather() + jb_im2col_u8.  An evicted reference gives zero rows and makes the next check() raise."""
+        if idx is not None and (idx.dtype != torch.int32 or not idx.is_contiguous()):
+            raise ValueError(f"expected contiguous int32 row indices, got {idx.dtype}")
+        s = self.store
+        C.jb_im2col_u8_frames(ptr(s.frames), ptr(s.first), ptr(s.head), s.F, s.n, ptr(self.refs), ptr(idx), M, ptr(col),
+                              ptr(s.status), stream_ptr())
+        return col
 
 
 def attach(env, memory, n_step):

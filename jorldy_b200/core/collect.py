@@ -7,30 +7,40 @@ randomness).
 """
 import torch
 
-from .buffer import DeviceRollout, frame_store
+from .buffer import DeviceRollout, FrameRollout, frame_store
 
 
 class RolloutCollector:
     def __init__(self, env, agent, n_step=None, use_cuda_graph=True):
         self.env, self.agent = env, agent
         self.T = n_step or agent.n_step
-        self.rollout = DeviceRollout(env.num_envs, self.T, env.state_size, env.action_size, env.action_type,
-                                     device=agent.device)
+        # Atari-shaped envs: every frame is pushed once and the rollout stores frame references (buffer/frame_store.py)
+        self.frames = bool(getattr(env, "frame_stack", False))
+        if self.frames:
+            self.rollout = FrameRollout(env.num_envs, self.T, env.action_size, env.action_type, device=agent.device)
+        else:
+            self.rollout = DeviceRollout(env.num_envs, self.T, env.state_size, env.action_size, env.action_type,
+                                         device=agent.device)
         self.use_cuda_graph = use_cuda_graph
         self._graph = None
         # kernels of OUR library per env step: mlp_in_fwd + gemm + heads_fwd + act + env_step (the
         # rollout-row copies are torch plumbing and not counted)
         self.launches_per_collect = 5 * self.T
         env.reset_device()
+        if self.frames:
+            self.rollout.start(env.obs)
 
     def _collect_eager(self):
         env, agent, ro = self.env, self.agent, self.rollout
         ro.clear()
         for t in range(self.T):
-            ro.state[:, t].copy_(env.obs)                      # state acted on (pre-step observation)
+            if not self.frames:
+                ro.state[:, t].copy_(env.obs)                  # state acted on (pre-step observation)
             action = agent.act_device(env.obs, training=True)
             next_obs, reward, done = env.step_device(action)   # env.obs <- post-reset observation
             ro.t = t
+            if self.frames:
+                next_obs = ro.push(env.obs, next_obs, done, env.auto_reset)
             ro.write_after_step(action, reward, done, next_obs)
 
     def collect(self):

@@ -71,17 +71,25 @@ class CNNHead:
             p[f"head.{name}.bias"].zero_()
 
     def forward(self, net, x, idx, M, tag, save):
-        if idx is not None:
-            x = x.index_select(0, idx.to(torch.int64))
-        if x.dtype != torch.uint8:
-            x = x.to(torch.uint8)
-        x = x.contiguous()
+        """x: a tensor of stacks, or a frame-ring row source (buffer/frame_store.py FrameRows) whose im2col fills conv1's
+        column matrix straight from the ring; rows idx[M] (int32) or all of them."""
+        rows = None if torch.is_tensor(x) else x
+        if rows is not None and self.D_in != tuple(rows.shape[1:]):
+            raise ValueError(f"a frame-ring input is {tuple(rows.shape[1:])}, this head takes {self.D_in}")
+        if rows is None:
+            if idx is not None:
+                x = x.index_select(0, idx.to(torch.int64))
+            if x.dtype != torch.uint8:
+                x = x.to(torch.uint8)
+            x = x.contiguous()
         s = stream_ptr()
         cur = None
         for li, (name, ci, co, k, st, (ih, iw), (oh, ow)) in enumerate(self.layers):
             K = ci * k * k
             col = net._buf(f"{tag}head.col{li}", (M * oh * ow, K))
-            if li == 0:
+            if li == 0 and rows is not None:
+                rows.im2col(idx, M, col)
+            elif li == 0:
                 C.jb_im2col_u8(ptr(x), M, ci, ih, iw, k, k, st, ptr(col), s)
             else:
                 C.jb_im2col_nhwc(ptr(cur), M, ci, ih, iw, k, k, st, ptr(col), s)

@@ -15,6 +15,8 @@
 // Gather (grid = sample x {state, next} x stack slot, one contiguous 7056-byte frame per CTA): a reference whose frames
 // are no longer resident (an overwritten slot) is never read: its output is zeroed and *status is set, for the host to
 // raise on.  At B = 32..512 the gather moves 0.9..14 MB and is launch-latency-bound.
+// PPO's frame rollout keeps its states on the same rings; im2col_u8_frames_kernel below writes conv1's column matrix
+// straight from them, with the gather's stack rule and residency check.
 #include "common.cuh"
 
 namespace {
@@ -93,6 +95,56 @@ __global__ void frame_gather_kernel(const uint8_t* __restrict__ frames, const in
   }
 }
 
+// conv1's im2col (8x8 kernel, stride 4, 4x84x84 -> 20x20 outputs, K = 256 in im2col_u8_nchw_vec4_kernel's order
+// c*64 + ky*8 + kx) read straight from the ring: grid = (stack i, output row oy), 256 threads.  Four threads resolve the
+// stack's four source frames (the stack rule and residency check of frame_gather_kernel) into shared memory; then each
+// thread turns one 4-byte frame-row load into one 16-byte column store, five times: 20 x 64 float4 = 20 KB per CTA.
+constexpr int OUT = 20, KSZ = 8, STRIDE = 4, K4 = STACK * KSZ * KSZ / 4;
+constexpr int ROW_VEC = OUT * K4;                  // float4 of one output row oy of one stack
+
+__global__ void __launch_bounds__(256) im2col_u8_frames_kernel(
+    const uint8_t* __restrict__ frames, const int64_t* __restrict__ first, const int64_t* __restrict__ head, long long F,
+    int n_lanes, const int64_t* __restrict__ refs, const int32_t* __restrict__ idx, float* __restrict__ col,
+    int32_t* __restrict__ status) {
+  __shared__ long long src[STACK];               // frame index lane * F + slot, or -1 when the stack is not resident
+  const long long i = blockIdx.x;
+  const int oy = blockIdx.y;
+  if (threadIdx.x < STACK) {
+    const int k = threadIdx.x;
+    const long long r = refs[idx ? idx[i] : i];
+    const long long lane = r >> POS_BITS, p = r & POS_MASK;
+    bool ok = r >= 0 && lane < n_lanes;
+    long long s = -1;
+    if (ok) {
+      const long long h = head[lane];
+      ok = p < h && p >= h - F;
+      if (ok) {
+        const long long f = first[lane * F + p % F];
+        const long long lo = p - 3 > f ? p - 3 : f;
+        ok = lo >= h - F && f <= p;
+        const long long q = p - 3 + k > f ? p - 3 + k : f;
+        s = ok ? lane * F + q % F : -1;
+      }
+    }
+    src[k] = s;
+    if (!ok && k == 0 && oy == 0) *reinterpret_cast<volatile int32_t*>(status) = 1;
+  }
+  __syncthreads();
+  float4* out = reinterpret_cast<float4*>(col) + ((size_t)i * OUT + oy) * ROW_VEC;
+  for (int q = threadIdx.x; q < ROW_VEC; q += blockDim.x) {
+    const int ox = q / K4, k4 = q % K4;
+    const int kx4 = k4 & 1, ky = (k4 >> 1) & (KSZ - 1), c = k4 >> 4;
+    const long long s = src[c];
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (s >= 0) {
+      const uchar4 u = *reinterpret_cast<const uchar4*>(frames + (size_t)s * FRAME + (oy * STRIDE + ky) * 84 +
+                                                         ox * STRIDE + 4 * kx4);
+      v = make_float4((float)u.x / 255.0f, (float)u.y / 255.0f, (float)u.z / 255.0f, (float)u.w / 255.0f);
+    }
+    out[q] = v;
+  }
+}
+
 }  // namespace
 
 JB_API int jb_frame_push(uint8_t* frames, int64_t* first, int64_t* head, int64_t frames_per_lane, const uint8_t* obs,
@@ -113,5 +165,16 @@ JB_API int jb_frame_gather(const uint8_t* frames, const int64_t* first, const in
   frame_gather_kernel<<<dim3(B, 2, STACK), 128, 0, (cudaStream_t)stream>>>(frames, first, head, frames_per_lane, n_lanes,
                                                                             state_refs, next_refs, idx, state_out, next_out,
                                                                             status);
+  return jb_check_launch();
+}
+
+JB_API int jb_im2col_u8_frames(const uint8_t* frames, const int64_t* first, const int64_t* head, int64_t frames_per_lane,
+                               int n_lanes, const int64_t* refs, const int32_t* idx, int M, float* col, int32_t* status,
+                               void* stream) {
+  if (!frames || !first || !head || !refs || !col || !status || M <= 0 || n_lanes <= 0 ||
+      frames_per_lane < 8 || (((uintptr_t)frames & 3) | ((uintptr_t)col & 15)))
+    return JB_ERR_INVALID;
+  im2col_u8_frames_kernel<<<dim3(M, OUT), 256, 0, (cudaStream_t)stream>>>(frames, first, head, frames_per_lane, n_lanes,
+                                                                           refs, idx, col, status);
   return jb_check_launch();
 }
