@@ -271,4 +271,22 @@ JB_API int jb_sac_actor_bwd(const float* raw, int nout, const float* eps, const 
 JB_API int jb_sac_alpha(const float* log_alpha, const float* stats4, float* alpha, float* grad, float* alpha_loss,
                         void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Discrete-action SAC (SAC-Discrete, arXiv:1910.07207), A <= 18 actions; logpi = log_softmax(logits), pi = exp(logpi).
+ *   jb_sacd_act          a ~ Categorical(pi) by inverse CDF on u[m] (NULL: Philox(seed, stream_base + m, row_ctr[m]++));
+ *                        greedy: argmax pi, first index on ties; action int64 [M]
+ *   jb_sacd_critic_loss  y = r + ((1-d) gamma) sum_a pi'(a)[min(nq1,nq2)(a) - alpha logpi'(a)] with pi' from next_logits;
+ *                        dq_i[b,a_b] = 2(Q_i(s)[a_b] - y)/B, 0 elsewhere; stats = {mse1, mse2, max y}
+ *   jb_sacd_actor        f = alpha logpi - min(q1,q2), L_b = sum_a pi f, dlogits = pi (f - L_b)/B;
+ *                        stats4 = {mean L, mean sum_a pi min(q1,q2), mean H, mean H - target_entropy}, H = -sum_a pi logpi
+ * The two loss kernels run one CTA with fixed-order reductions, so a learn() is bit-reproducible.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_sacd_act(const float* logits, int M, int A, const float* u, uint64_t seed, uint64_t stream_base,
+                       long long* row_ctr, int greedy, int64_t* action, void* stream);
+JB_API int jb_sacd_critic_loss(const float* q1, const float* q2, const float* nq1, const float* nq2, const float* next_logits,
+                               const int64_t* action, const float* reward, const float* done, const float* alpha, int B,
+                               int A, float gamma, float* dq1, float* dq2, float* stats, void* stream);
+JB_API int jb_sacd_actor(const float* logits, const float* q1, const float* q2, const float* alpha, float target_entropy,
+                         int B, int A, float* dlogits, float* stats4, void* stream);
+
 #endif /* JORLDY_B200_H */

@@ -4,7 +4,8 @@
 config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / train).  Values follow the
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
 per, noisy, c51, rainbow, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar / pendulum / atari(synthetic) /
-mujoco(synthetic dims); an existing JORLDY config directory on sys.path takes precedence
+mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
+which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -143,10 +144,28 @@ def _ac_config(agent, env):
     return dict(env=env_d, agent=a, optim=opt, train=tr)
 
 
+def _sac_discrete_config(env):
+    """Discrete-action SAC (agent name "sac", actor "discrete_policy").  These follow the SAC-Discrete paper
+    (Christodoulou 2019, arXiv:1910.07207), not a reference config file; a JORLDY config directory on sys.path takes
+    precedence.  cartpole: config.sac.cartpole with the discrete actor and critic.  atari names no game: runs pass
+    --env.name."""
+    if env == "cartpole":
+        d = _ac_config("sac", "cartpole")
+        d["env"].update(action_type="discrete")
+        d["agent"].update(actor="discrete_policy", critic="discrete_q_network")
+        return d
+    a = dict(name="sac", actor="discrete_policy", critic="discrete_q_network", head="cnn", use_dynamic_alpha=True, gamma=0.99,
+             tau=5e-3, buffer_size=1000000, batch_size=64, start_train_step=20000)
+    return dict(env=dict(_ATARI_ENV), agent=a,
+                optim=dict(actor="adam", critic="adam", alpha="adam", actor_lr=3e-4, critic_lr=3e-4, alpha_lr=3e-4),
+                train=dict(_TRAIN_ATARI, update_period=4, num_workers=16))
+
+
 def available():
     out = []
     for ag, envs in _AC_ENVS.items():
         out += [f"config.{ag}.{e}" for e in envs]
+    out += [f"config.sac_discrete.{e}" for e in ("cartpole", "atari")]
     for ag in list(_VALUE_AGENTS) + ["ape_x"]:
         out += [f"config.{ag}.{e}" for e in ("cartpole", "mountaincar", "atari")]
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
@@ -166,6 +185,8 @@ def load(config_path):
         d = _ppo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
+    elif agent == "sac_discrete" and env in ("cartpole", "atari"):
+        d = _sac_discrete_config(env)
     else:
         raise ImportError(f"no config '{config_path}' (built-ins: {available()})")
     return SimpleNamespace(**d)

@@ -1,4 +1,5 @@
-"""Continuous off-policy actor-critic agents on the GPU-resident pipeline: DDPG, TD3 and SAC (continuous actions).
+"""Off-policy actor-critic agents on the GPU-resident pipeline: DDPG, TD3 and SAC (continuous actions), and the
+discrete-action SAC (SACDiscrete, selected by SAC's `actor="discrete_policy"`).
 
 Mirrors jorldy/core/agent/{ddpg,td3,sac}.py: same constructor kwargs, optimiser layout (one optimiser per network),
 bookkeeping (soft target updates, TD3's delayed actor update, SAC's one-step-lagged alpha) and result keys.
@@ -355,15 +356,23 @@ class TD3(DDPG):
 
 
 class SAC(_ActorCritic):
-    """jorldy/core/agent/sac.py:16-355, continuous actions (`actor="continuous_policy"`)."""
+    """jorldy/core/agent/sac.py:16-355, continuous actions (`actor="continuous_policy"`); `actor="discrete_policy"`
+    constructs the discrete-action SAC (SACDiscrete below)."""
     _n_critics = 2
+    _actor_kind = "continuous"
+
+    def __new__(cls, *args, **kwargs):
+        actor = kwargs.get("actor", args[3] if len(args) > 3 else "continuous_policy")
+        if cls is SAC and actor.split("_")[0] == "discrete":
+            cls = SACDiscrete
+        return super().__new__(cls)
 
     def __init__(self, state_size, action_size, hidden_size=512, actor="continuous_policy", critic="continuous_q_network",
                  head="mlp", optim_config=dict(_DEFAULT_OPTIM, alpha="adam", alpha_lr=3e-4), use_dynamic_alpha=False,
                  gamma=0.99, tau=5e-3, buffer_size=50000, batch_size=64, start_train_step=2000, static_log_alpha=-2.0,
                  target_update_period=10000, run_step=1e6, lr_decay=True, device=None, seed=0, use_cuda_graph=True, **kwargs):
-        if actor.split("_")[0] != "continuous":
-            raise NotImplementedError("only the continuous-action SAC (config/sac/{pendulum,mujoco,...}.py) is built here")
+        if actor.split("_")[0] != self._actor_kind:
+            raise NotImplementedError(f"actor '{actor}': SAC is built with continuous_policy and discrete_policy actors")
         self._common(state_size, action_size, hidden_size, actor, critic, head, optim_config, gamma, buffer_size, batch_size,
                      start_train_step, tau, run_step, lr_decay, device, seed, target_actor=False, use_cuda_graph=use_cuda_graph)
         self.use_dynamic_alpha = use_dynamic_alpha
@@ -464,3 +473,77 @@ class SAC(_ActorCritic):
         if self.use_dynamic_alpha and "log_alpha" in ck:
             self.log_alpha.flat[:1].copy_(torch.as_tensor(ck["log_alpha"]).detach().reshape(1).to(self.device))
             self.alpha_optimizer.load_state_dict(ck["alpha_optimizer"])
+
+
+class SACDiscrete(SAC):
+    """SAC with a categorical policy (`actor="discrete_policy"`, `critic="discrete_q_network"`): SAC-Discrete
+    (Christodoulou 2019, arXiv:1910.07207) with the continuous SAC's bookkeeping: soft target update on every process()
+    once learning has started, alpha from before the previous learn's log_alpha step, the checkpoint layout and its
+    critic2 -> critic1 load.  The policy's expectations over the A actions are exact, so a learn() draws no noise:
+
+        target   V' = sum_a pi'(a) [min(Q1', Q2')(s', a) - alpha logpi'(a)],  y = r + (1 - d) gamma V'
+        critics  L_i = mean (Q_i(s)[a] - y)^2
+        actor    L = mean_b sum_a pi(a) [alpha logpi(a) - min(Q1, Q2)(s, a)], through the updated critics
+        alpha    alpha_loss = log_alpha * mean(H - target_entropy), H = -sum_a pi logpi, target_entropy = 0.98 ln A
+
+    Actions are int64 [N, 1]; with the cnn head, states stay uint8 stacks (the head scales by 1/255)."""
+    action_type = "discrete"
+    _actor_kind = "discrete"
+
+    def __init__(self, *args, **kwargs):
+        if len(args) < 4:
+            kwargs.setdefault("actor", "discrete_policy")
+        if len(args) < 5:
+            kwargs.setdefault("critic", "discrete_q_network")
+        super().__init__(*args, **kwargs)
+        self.target_entropy = 0.98 * float(np.log(self.action_size))
+
+    def _net_input(self, s):
+        return s if s.dtype == torch.uint8 else s.to(torch.float32).reshape(s.shape[0], -1)
+
+    def _unpack(self, batch):
+        B = batch["reward"].shape[0]
+        f = lambda k: batch[k].to(torch.float32).reshape(B).contiguous()
+        a = batch["action"].reshape(B).to(torch.int64).contiguous()
+        return B, self._net_input(batch["state"]), a, f("reward"), f("done"), self._net_input(batch["next_state"])
+
+    def act_device(self, state, training=True, noise=None):
+        """a ~ Categorical(softmax(actor(s))) when training, argmax otherwise; noise: optional f32 [N] uniforms in [0, 1)."""
+        M, A = state.shape[0], self.action_size
+        logits = self.actor._buf("act.z", (M, A))
+        self.actor.forward_rows(state, logits)
+        if M not in self._row_ctr:
+            self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        action = self.actor._buf("act.a", (M, 1), torch.int64)
+        C.jb_sacd_act(ptr(logits), M, A, ptr(noise), self.seed, self.rng_stream_base, ptr(self._row_ctr[M]),
+                      0 if training else 1, ptr(action), stream_ptr())
+        return action, None
+
+    def _learn_core(self, batch):
+        B, s, a, r, d, ns = self._unpack(batch)
+        A, st, sp = self.action_size, self._stats, stream_ptr()
+        c1, c2 = self.critics
+        q1, q2 = c1.forward(s, tag="t."), c2.forward(s, tag="t.")
+        nz = self.actor.forward_raw(ns, tag="n.", save=False)
+        nq1 = self.target_critics[0].forward(ns, tag="n.", save=False)
+        nq2 = self.target_critics[1].forward(ns, tag="n.", save=False)
+        dq1, dq2 = c1._buf("t.dq", (B, A)), c2._buf("t.dq", (B, A))
+        C.jb_sacd_critic_loss(ptr(q1), ptr(q2), ptr(nq1), ptr(nq2), ptr(nz), ptr(a), ptr(r), ptr(d), ptr(self.alpha), B, A,
+                              self.gamma, ptr(dq1), ptr(dq2), ptr(st), sp)
+        self._critic_step(0, dq1, B)
+        self._critic_step(1, dq2, B)
+        z = self.actor.forward_raw(s, tag="t.")
+        qa1, qa2 = c1.forward(s, tag="a.", save=False), c2.forward(s, tag="a.", save=False)
+        dz = self.actor._buf("t.dz", (B, A))
+        C.jb_sacd_actor(ptr(z), ptr(qa1), ptr(qa2), ptr(self.alpha), self.target_entropy, B, A, ptr(dz), st.data_ptr() + 16, sp)
+        self.actor.backward_raw(dz, B, tag="t.")
+        self.actor_optimizer.step()
+        C.jb_sac_alpha(ptr(self.log_alpha.flat), st.data_ptr() + 16, ptr(self.alpha), ptr(self.log_alpha.grad),
+                       st.data_ptr() + 32, sp)
+        if self.use_dynamic_alpha:
+            self.alpha_optimizer.step()
+
+    def _finish(self):
+        result = super()._finish()
+        self.memory.check_frames()
+        return result

@@ -5,7 +5,7 @@ from collections import OrderedDict
 from .policy_value import DiscretePolicyValue, ContinuousPolicyValue, DiscreteQ_Network
 from .dueling import Dueling
 from .noisy import Noisy, Rainbow
-from .policy import ContinuousPolicy, DeterministicPolicy
+from .policy import ContinuousPolicy, DeterministicPolicy, DiscretePolicy
 from .q_network import ContinuousQ_Network
 
 network_dict = OrderedDict(
@@ -13,6 +13,7 @@ network_dict = OrderedDict(
     continuous_policy_value=ContinuousPolicyValue,
     continuous_q_network=ContinuousQ_Network,
     deterministic_policy=DeterministicPolicy,
+    discrete_policy=DiscretePolicy,
     discrete_policy_value=DiscretePolicyValue,
     discrete_q_network=DiscreteQ_Network,
     dueling=Dueling,

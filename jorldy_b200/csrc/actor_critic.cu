@@ -266,6 +266,139 @@ __global__ void sac_alpha_kernel(const float* __restrict__ log_alpha, const floa
   }
 }
 
+// ---- discrete-action SAC (SAC-Discrete, Christodoulou 2019, arXiv:1910.07207) --------------------------------------------
+// One row of A <= SACD_MAX_A logits per thread, held in registers: every loop over actions is fully unrolled and guarded
+// by `a < A`, so no per-thread array is indexed dynamically.  logpi = log_softmax(z) exactly (z - max - log sum exp),
+// pi = exp(logpi).
+constexpr int SACD_MAX_A = 18;   // the full Atari action set
+
+__device__ __forceinline__ void sacd_log_softmax(const float* __restrict__ z, int A, float (&lp)[SACD_MAX_A]) {
+  float mx = -INFINITY;
+#pragma unroll
+  for (int a = 0; a < SACD_MAX_A; ++a) if (a < A) { lp[a] = z[a]; mx = fmaxf(mx, lp[a]); }
+  float s = 0.f;
+#pragma unroll
+  for (int a = 0; a < SACD_MAX_A; ++a) if (a < A) s += expf(lp[a] - mx);
+  const float lse = mx + logf(s);
+#pragma unroll
+  for (int a = 0; a < SACD_MAX_A; ++a) if (a < A) lp[a] = lp[a] - lse;
+}
+
+// act: a ~ Categorical(pi) by inverse CDF on one uniform per row (u_in, or Philox(seed, stream_base + m, row_ctr[m]) with
+// the row's counter advanced, so CUDA-graph replays draw fresh numbers); greedy: argmax pi, first index on ties.
+__global__ void sacd_act_kernel(const float* __restrict__ z, int M, int A, const float* __restrict__ u_in, uint64_t seed,
+                                uint64_t stream_base, long long* __restrict__ row_ctr, int greedy,
+                                int64_t* __restrict__ action) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  float lp[SACD_MAX_A];
+  sacd_log_softmax(z + (size_t)m * A, A, lp);
+  int pick = 0;
+  if (greedy) {
+    float best = -1.f;
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a)
+      if (a < A) { const float p = expf(lp[a]); if (p > best) { best = p; pick = a; } }
+  } else {
+    float u;
+    if (u_in) u = u_in[m];
+    else {
+      uint64_t ctr = 0;
+      if (row_ctr) { ctr = (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
+      u = jb_u01_float(jb_philox(seed, stream_base + (uint64_t)m, ctr).x);
+    }
+    float tot = 0.f;
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a) if (a < A) tot += expf(lp[a]);
+    const float target = u * tot;
+    float c = 0.f;
+    pick = A - 1;
+    bool found = false;
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a)
+      if (a < A && !found) { c += expf(lp[a]); if (target < c) { pick = a; found = true; } }
+  }
+  action[m] = pick;
+}
+
+// critics: V' = sum_a pi'(a) [min(nq1, nq2)(a) - alpha logpi'(a)]   (pi' from the actor on s', nq_i the target critics)
+//          y = r + ((1 - d) gamma) V';  q_i = Q_i(s)[a_b];  loss_i = mean (q_i - y)^2
+//          dq_i[b,k] = 2 (q_i - y) / B at k = a_b, 0 elsewhere;  stats = {loss1, loss2, max_b y}
+__global__ void __launch_bounds__(256) sacd_critic_loss_kernel(
+    const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ nq1, const float* __restrict__ nq2,
+    const float* __restrict__ nz, const int64_t* __restrict__ action, const float* __restrict__ reward,
+    const float* __restrict__ done, const float* __restrict__ alpha, int B, int A, float gamma, float* __restrict__ dq1,
+    float* __restrict__ dq2, float* __restrict__ stats) {
+  __shared__ float sm[9];
+  float s1 = 0.f, s2 = 0.f, mx = -INFINITY;
+  const float inv = 1.f / (float)B, al = alpha[0];
+  for (int b = threadIdx.x; b < B; b += 256) {
+    const size_t o = (size_t)b * A;
+    float lp[SACD_MAX_A];
+    sacd_log_softmax(nz + o, A, lp);
+    float v = 0.f;
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a)
+      if (a < A) v += expf(lp[a]) * (fminf(nq1[o + a], nq2[o + a]) - al * lp[a]);
+    const float y = __fadd_rn(reward[b], __fmul_rn(__fmul_rn(1.f - done[b], gamma), v));
+    mx = fmaxf(mx, y);
+    const int k = (int)action[b];
+    const float e1 = q1[o + k] - y, e2 = q2[o + k] - y;
+    s1 += e1 * e1;
+    s2 += e2 * e2;
+    for (int a = 0; a < A; ++a) {
+      dq1[o + a] = a == k ? 2.f * e1 * inv : 0.f;
+      dq2[o + a] = a == k ? 2.f * e2 * inv : 0.f;
+    }
+  }
+  s1 = block_sum256(s1, sm);
+  s2 = block_sum256(s2, sm);
+  mx = block_max256(mx, sm);
+  if (threadIdx.x == 0) { stats[0] = s1 * inv; stats[1] = s2 * inv; stats[2] = mx; }
+}
+
+// actor, through the updated critics: m = min(q1, q2) over [B,A], f = alpha logpi - m, L_b = sum_a pi f,
+// actor_loss = mean_b L_b, dz[b,k] = pi_k (f_k - L_b) / B.  H_b = -sum_a pi logpi.
+// stats = {actor_loss, mean_b sum_a pi m, mean H, mean H - target_entropy}.
+__global__ void __launch_bounds__(256) sacd_actor_kernel(const float* __restrict__ z, const float* __restrict__ q1,
+                                                         const float* __restrict__ q2, const float* __restrict__ alpha,
+                                                         float target_entropy, int B, int A, float* __restrict__ dz,
+                                                         float* __restrict__ stats) {
+  __shared__ float sm[9];
+  float sl = 0.f, sq = 0.f, se = 0.f;
+  const float inv = 1.f / (float)B, al = alpha[0];
+  for (int b = threadIdx.x; b < B; b += 256) {
+    const size_t o = (size_t)b * A;
+    float lp[SACD_MAX_A], f[SACD_MAX_A];
+    sacd_log_softmax(z + o, A, lp);
+    float L = 0.f, mq = 0.f, H = 0.f;
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a)
+      if (a < A) {
+        const float p = expf(lp[a]), m = fminf(q1[o + a], q2[o + a]);
+        f[a] = al * lp[a] - m;
+        L += p * f[a];
+        mq += p * m;
+        H -= p * lp[a];
+      }
+#pragma unroll
+    for (int a = 0; a < SACD_MAX_A; ++a)
+      if (a < A) dz[o + a] = expf(lp[a]) * (f[a] - L) * inv;
+    sl += L;
+    sq += mq;
+    se += H;
+  }
+  sl = block_sum256(sl, sm);
+  sq = block_sum256(sq, sm);
+  se = block_sum256(se, sm);
+  if (threadIdx.x == 0) {
+    stats[0] = sl * inv;
+    stats[1] = sq * inv;
+    stats[2] = se * inv;
+    stats[3] = se * inv - target_entropy;
+  }
+}
+
 }  // namespace
 
 JB_API int jb_soft_update(float* target, const float* online, int64_t n, double tau, void* stream) {
@@ -346,5 +479,31 @@ JB_API int jb_sac_alpha(const float* log_alpha, const float* stats4, float* alph
                         void* stream) {
   if (!log_alpha || !stats4 || !alpha || !alpha_loss) return JB_ERR_INVALID;
   sac_alpha_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(log_alpha, stats4, alpha, grad, alpha_loss);
+  return jb_check_launch();
+}
+
+JB_API int jb_sacd_act(const float* logits, int M, int A, const float* u, uint64_t seed, uint64_t stream_base,
+                       long long* row_ctr, int greedy, int64_t* action, void* stream) {
+  if (!logits || !action || M <= 0 || A <= 0 || A > SACD_MAX_A) return JB_ERR_INVALID;
+  sacd_act_kernel<<<jb_div_up(M, 128), 128, 0, (cudaStream_t)stream>>>(logits, M, A, u, seed, stream_base, row_ctr, greedy,
+                                                                       action);
+  return jb_check_launch();
+}
+
+JB_API int jb_sacd_critic_loss(const float* q1, const float* q2, const float* nq1, const float* nq2, const float* next_logits,
+                               const int64_t* action, const float* reward, const float* done, const float* alpha, int B,
+                               int A, float gamma, float* dq1, float* dq2, float* stats, void* stream) {
+  if (!q1 || !q2 || !nq1 || !nq2 || !next_logits || !action || !reward || !done || !alpha || !dq1 || !dq2 || !stats ||
+      B <= 0 || A <= 0 || A > SACD_MAX_A)
+    return JB_ERR_INVALID;
+  sacd_critic_loss_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(q1, q2, nq1, nq2, next_logits, action, reward, done, alpha, B,
+                                                               A, gamma, dq1, dq2, stats);
+  return jb_check_launch();
+}
+
+JB_API int jb_sacd_actor(const float* logits, const float* q1, const float* q2, const float* alpha, float target_entropy,
+                         int B, int A, float* dlogits, float* stats4, void* stream) {
+  if (!logits || !q1 || !q2 || !alpha || !dlogits || !stats4 || B <= 0 || A <= 0 || A > SACD_MAX_A) return JB_ERR_INVALID;
+  sacd_actor_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(logits, q1, q2, alpha, target_entropy, B, A, dlogits, stats4);
   return jb_check_launch();
 }
