@@ -128,6 +128,7 @@ JB_API int jb_linear_io_bwd_dx(const float* dy, const float* w, float* dx, int M
                                const float* relu_act, void* stream);
 JB_API int jb_linear_io_bwd_dw(const float* dy, const float* x, float* dw, int M, int in_f, int out_f, void* stream);
 JB_API int jb_colsum(const float* x, int M, int N, float* out, int accumulate, void* stream);
+/* h1 = relu(x[idx] W1^T + b1) for 1 <= D <= 32 inputs (the synthetic control env's widest observation). */
 JB_API int jb_mlp_in_fwd(const float* x, const int32_t* idx, const float* w1, const float* b1, int M, int D, int H,
                          float* h1, float* xg, void* stream);
 JB_API int jb_heads_fwd(const float* h, int M, int H, const float* w0, const float* b0, int n0, const float* w1,
@@ -140,19 +141,23 @@ JB_API int jb_heads_bwd_dw(const float* dout, const float* h, int M, int H, floa
 /* ---------------------------------------------------------------------------------------------
  * PPO — jorldy/core/agent/ppo.py:54-69 (act), :83-93 (value / log_prob_old), :127-162 (loss).
  * `out` is the [M,nout] pre-activation head output: discrete [logits(A)|v], continuous
- * [mu(A)|log_std(A)|v].
+ * [mu(A)|log_std(A)|v].  A wider A than an entry point's bound returns JB_ERR_INVALID.
  * ------------------------------------------------------------------------------------------- */
+/* 1 <= A <= 18 (ALE's full action set) */
 JB_API int jb_ppo_act_discrete(const float* out, int M, int A, int nout, const float* u, uint64_t seed,
                                uint64_t stream_base, uint64_t ctr, long long* row_ctr, int greedy, int64_t* action,
                                void* stream);
+/* 1 <= A <= 8 */
 JB_API int jb_ppo_act_continuous(const float* out, int M, int A, int nout, const float* normal, uint64_t seed,
                                  uint64_t stream_base, uint64_t ctr, long long* row_ctr, int greedy, float* action,
                                  void* stream);
+/* 1 <= A <= 18 */
 JB_API int jb_ppo_prepass_discrete(const float* out, const int32_t* action, int M, int A, int nout, float* value,
                                    float* logp_old, void* stream);
 JB_API int jb_ppo_prepass_continuous(const float* out, const float* action, int M, int A, int nout, float* value,
                                      float* logp_old, void* stream);
 JB_API int jb_take_minibatch(const int32_t* perm, long long* cursor, int B, int32_t* cur_idx, void* stream);
+/* 1 <= A <= 18 discrete, 1 <= A <= 8 continuous */
 JB_API int jb_ppo_loss(int continuous, const float* out, const int32_t* idx, const void* action, const float* adv,
                        const float* ret, const float* value_old, const float* logp_old, int B, int A, int nout,
                        float eps_clip, float vf_coef, float ent_coef, float* dout, float* stats, float* acc,

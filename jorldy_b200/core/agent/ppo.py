@@ -22,6 +22,7 @@ from ..optimizer import Optimizer
 from .base import BaseAgent
 
 GRAPH_CHUNK = 16     # minibatch steps captured per CUDA graph
+MAX_ACTION_SIZE = {"discrete": 18, "continuous": 8}   # csrc/ppo_rowmath.cuh MAX_A_DISC / MAX_A
 
 
 class PPO(BaseAgent):
@@ -55,6 +56,9 @@ class PPO(BaseAgent):
         self.device = require_cuda(device)
         self.action_type = network.split("_")[0]
         assert self.action_type in ["continuous", "discrete"]
+        max_a = MAX_ACTION_SIZE[self.action_type]
+        if action_size > max_a:
+            raise ValueError(f"PPO's {self.action_type} kernels take at most {max_a} actions, got action_size={action_size}")
         self.state_size, self.action_size = state_size, action_size
         self.network = Network(network, state_size, action_size, D_hidden=hidden_size, head=head,
                                device=self.device)

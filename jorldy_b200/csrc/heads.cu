@@ -3,14 +3,14 @@
 //
 // Reference modules: jorldy/core/network/head.py:6-18 (MLP head: relu(Linear(D_in,H))),
 // policy_value.py:11-22,41-57 (pi/mu/log_std/v heads), q_network.py:13-20 (q head),
-// dueling.py:13-32 (l2_a / l2_v).  These layers have one tiny dimension (D_in = 4..11,
+// dueling.py:13-32 (l2_a / l2_v).  These layers have one tiny dimension (D_in = 1..32,
 // outputs = 1..8), so a tiled GEMM would waste >85 % of every tile; instead each is a
 // row-/element-parallel kernel that keeps HBM/L2 accesses coalesced along H.
 #include "common.cuh"
 
 namespace {
 
-constexpr int MAX_DIN = 16;
+constexpr int MAX_DIN = 32;    // the synthetic control env's widest observation (env_synth.cu MAX_D)
 constexpr int MAX_NOUT = 32;
 
 // h1[m, j] = relu(b1[j] + sum_i x[row(m), i] * W1[j, i]);  row(m) = idx ? idx[m] : m.

@@ -27,10 +27,13 @@
 namespace {
 
 using jbppo::MAX_A;
+using jbppo::MAX_A_DISC;
 using jbppo::log_softmax_row;
 using jbppo::atanh_clamped;
 
 // ---- act ------------------------------------------------------------------------------------
+// NA: compile-time bound on A (MAX_A or MAX_A_DISC); every loop runs to NA with an `a < A` guard so lg/lsm stay in registers
+template <int NA>
 __global__ void ppo_act_discrete_kernel(const float* __restrict__ out, int M, int A, int nout,
                                         const float* __restrict__ u_in, uint64_t seed, uint64_t stream_base,
                                         uint64_t ctr, long long* __restrict__ row_ctr, int greedy,
@@ -38,24 +41,29 @@ __global__ void ppo_act_discrete_kernel(const float* __restrict__ out, int M, in
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
   if (row_ctr) { ctr += (uint64_t)row_ctr[m]; row_ctr[m] += 1; }   // per-row draw counter (graph-replay safe)
-  float lg[MAX_A], lsm[MAX_A];
-  for (int a = 0; a < A; ++a) lg[a] = out[(size_t)m * nout + a];
-  log_softmax_row(lg, A, lsm);
+  float lg[NA], lsm[NA];
+#pragma unroll
+  for (int a = 0; a < NA; ++a) lg[a] = a < A ? out[(size_t)m * nout + a] : 0.f;
+  log_softmax_row<NA>(lg, A, lsm);
   int pick = 0;
   if (greedy) {
     float best = expf(lsm[0]);
-    for (int a = 1; a < A; ++a) { const float p = expf(lsm[a]); if (p > best) { best = p; pick = a; } }
+#pragma unroll
+    for (int a = 1; a < NA; ++a) if (a < A) { const float p = expf(lsm[a]); if (p > best) { best = p; pick = a; } }
   } else {
     float u;
     if (u_in) u = u_in[m];
     else { jb_philox4 r = jb_philox(seed, stream_base + (uint64_t)m, ctr); u = jb_u01_float(r.x); }
     // inverse CDF on pi = exp(log_softmax) (same law as torch.multinomial(pi, 1), ppo.py:64-68)
     float tot = 0.f;
-    for (int a = 0; a < A; ++a) tot += expf(lsm[a]);
+#pragma unroll
+    for (int a = 0; a < NA; ++a) if (a < A) tot += expf(lsm[a]);
     const float target = u * tot;
     float c = 0.f;
+    bool found = false;
     pick = A - 1;
-    for (int a = 0; a < A; ++a) { c += expf(lsm[a]); if (target < c) { pick = a; break; } }
+#pragma unroll
+    for (int a = 0; a < NA; ++a) if (a < A && !found) { c += expf(lsm[a]); if (target < c) { pick = a; found = true; } }
   }
   action[m] = pick;
 }
@@ -90,16 +98,21 @@ __global__ void ppo_act_continuous_kernel(const float* __restrict__ out, int M, 
 }
 
 // ---- pre-pass: value + log_prob_old ------------------------------------------------------------
+template <int NA>
 __global__ void ppo_prepass_discrete_kernel(const float* __restrict__ out, const int32_t* __restrict__ action,
                                             int M, int A, int nout, float* __restrict__ value,
                                             float* __restrict__ logp_old) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
-  float lg[MAX_A], lsm[MAX_A];
-  for (int a = 0; a < A; ++a) lg[a] = out[(size_t)m * nout + a];
-  log_softmax_row(lg, A, lsm);
+  float lg[NA], lsm[NA];
+#pragma unroll
+  for (int a = 0; a < NA; ++a) lg[a] = a < A ? out[(size_t)m * nout + a] : 0.f;
+  log_softmax_row<NA>(lg, A, lsm);
   const int a = action[m];
-  logp_old[m] = logf(expf(lsm[a]));            // pi.gather(1, a).log(), pi = exp(log_softmax)
+  float la = 0.f;                              // lsm[a] without a run-time register index
+#pragma unroll
+  for (int q = 0; q < NA; ++q) if (q == a) la = lsm[q];
+  logp_old[m] = logf(expf(la));                // pi.gather(1, a).log(), pi = exp(log_softmax)
   value[m] = out[(size_t)m * nout + A];
 }
 
@@ -141,8 +154,10 @@ __device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
   __syncthreads();
 }
 
-template <bool CONT>
-__global__ void __launch_bounds__(256)
+// NA: compile-time bound on A, see jbppo::row.  The 18-wide row holds ~145 live registers: min-blocks 1 lets ptxas use
+// them instead of spilling at its default 128 (0 leaves the 8-wide instantiations unconstrained, as before).
+template <bool CONT, int NA>
+__global__ void __launch_bounds__(256, NA > MAX_A ? 1 : 0)
 ppo_loss_kernel(const float* __restrict__ out, const int32_t* __restrict__ idx, const void* __restrict__ action_all,
                 const float* __restrict__ adv_all, const float* __restrict__ ret_all,
                 const float* __restrict__ vold_all, const float* __restrict__ logp_old_all, int B, int A, int nout,
@@ -170,15 +185,16 @@ ppo_loss_kernel(const float* __restrict__ out, const int32_t* __restrict__ idx, 
   float max_ratio = -INFINITY, min_prob = INFINITY;
   if (b < B) {
     const int r = idx ? idx[b] : b;
-    jbppo::RowOut ro;
+    jbppo::RowOutW<jbppo::width<NA>()> ro;
     const float* o = out + (size_t)b * nout;
-    if (CONT) jbppo::row<true>(o, A, 0, (const float*)action_all + (size_t)r * A, adv_all[r], ret_all[r], vold_all[r],
+    if constexpr (CONT) jbppo::row<true, NA>(o, A, 0, (const float*)action_all + (size_t)r * A, adv_all[r], ret_all[r], vold_all[r],
                                logp_old_all + (size_t)r * A, hp, invB, ro);
-    else jbppo::row<false>(o, A, ((const int32_t*)action_all)[r], nullptr, adv_all[r], ret_all[r], vold_all[r],
+    else jbppo::row<false, NA>(o, A, ((const int32_t*)action_all)[r], nullptr, adv_all[r], ret_all[r], vold_all[r],
                            logp_old_all + r, hp, invB, ro);
     float* g = dout + (size_t)b * nout;
     const int npol = CONT ? 2 * A : A;
-    for (int a = 0; a < npol; ++a) g[a] = ro.dpol[a];
+#pragma unroll
+    for (int a = 0; a < (CONT ? 2 * NA : NA); ++a) if (a < npol) g[a] = ro.dpol[a];
     g[npol] = w1 * ro.dv1 + w2 * ro.dv2;
     st[0] = ro.surr_min; st[1] = ro.ent;
     max_ratio = ro.ratio; min_prob = ro.pmin;
@@ -243,8 +259,11 @@ JB_API int jb_take_minibatch(const int32_t* perm, long long* cursor, int B, int3
 JB_API int jb_ppo_act_discrete(const float* out, int M, int A, int nout, const float* u, uint64_t seed,
                                uint64_t stream_base, uint64_t ctr, long long* row_ctr, int greedy, int64_t* action,
                                void* stream) {
-  if (!out || !action || M <= 0 || A <= 0 || A > MAX_A || nout < A) return JB_ERR_INVALID;
-  ppo_act_discrete_kernel<<<jb_div_up(M, 128), 128, 0, (cudaStream_t)stream>>>(out, M, A, nout, u, seed, stream_base, ctr, row_ctr, greedy, action);
+  if (!out || !action || M <= 0 || A <= 0 || A > MAX_A_DISC || nout < A) return JB_ERR_INVALID;
+  const dim3 grid(jb_div_up(M, 128));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (A <= MAX_A) ppo_act_discrete_kernel<MAX_A><<<grid, 128, 0, s>>>(out, M, A, nout, u, seed, stream_base, ctr, row_ctr, greedy, action);
+  else ppo_act_discrete_kernel<MAX_A_DISC><<<grid, 128, 0, s>>>(out, M, A, nout, u, seed, stream_base, ctr, row_ctr, greedy, action);
   return jb_check_launch();
 }
 
@@ -258,8 +277,11 @@ JB_API int jb_ppo_act_continuous(const float* out, int M, int A, int nout, const
 
 JB_API int jb_ppo_prepass_discrete(const float* out, const int32_t* action, int M, int A, int nout, float* value,
                                    float* logp_old, void* stream) {
-  if (!out || !action || !value || !logp_old || M <= 0 || A <= 0 || A > MAX_A || nout != A + 1) return JB_ERR_INVALID;
-  ppo_prepass_discrete_kernel<<<jb_div_up(M, 128), 128, 0, (cudaStream_t)stream>>>(out, action, M, A, nout, value, logp_old);
+  if (!out || !action || !value || !logp_old || M <= 0 || A <= 0 || A > MAX_A_DISC || nout != A + 1) return JB_ERR_INVALID;
+  const dim3 grid(jb_div_up(M, 128));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (A <= MAX_A) ppo_prepass_discrete_kernel<MAX_A><<<grid, 128, 0, s>>>(out, action, M, A, nout, value, logp_old);
+  else ppo_prepass_discrete_kernel<MAX_A_DISC><<<grid, 128, 0, s>>>(out, action, M, A, nout, value, logp_old);
   return jb_check_launch();
 }
 
@@ -280,12 +302,13 @@ JB_API int jb_ppo_loss(int continuous, const float* out, const int32_t* idx, con
                        float eps_clip, float vf_coef, float ent_coef, float* dout, float* stats, float* acc,
                        void* stream) {
   if (!out || !action || !adv || !ret || !value_old || !logp_old || !dout || !stats) return JB_ERR_INVALID;
-  if (B <= 0 || A <= 0 || A > MAX_A || nout != (continuous ? 2 * A + 1 : A + 1)) return JB_ERR_INVALID;
+  if (B <= 0 || A <= 0 || A > (continuous ? MAX_A : MAX_A_DISC) || nout != (continuous ? 2 * A + 1 : A + 1)) return JB_ERR_INVALID;
   jbppo::HP hp{eps_clip, vf_coef, ent_coef};
   const int n_cta = jb_div_up(B, 256);
   cudaStream_t s = (cudaStream_t)stream;
-  if (continuous) ppo_loss_kernel<true><<<n_cta, 256, 0, s>>>(out, idx, action, adv, ret, value_old, logp_old, B, A, nout, hp, dout, stats);
-  else ppo_loss_kernel<false><<<n_cta, 256, 0, s>>>(out, idx, action, adv, ret, value_old, logp_old, B, A, nout, hp, dout, stats);
+  if (continuous) ppo_loss_kernel<true, MAX_A><<<n_cta, 256, 0, s>>>(out, idx, action, adv, ret, value_old, logp_old, B, A, nout, hp, dout, stats);
+  else if (A <= MAX_A) ppo_loss_kernel<false, MAX_A><<<n_cta, 256, 0, s>>>(out, idx, action, adv, ret, value_old, logp_old, B, A, nout, hp, dout, stats);
+  else ppo_loss_kernel<false, MAX_A_DISC><<<n_cta, 256, 0, s>>>(out, idx, action, adv, ret, value_old, logp_old, B, A, nout, hp, dout, stats);
   ppo_stats_finalize_kernel<<<1, 32, 0, s>>>(stats, n_cta, B, A, continuous, acc);
   return jb_check_launch();
 }

@@ -9,24 +9,31 @@
 
 namespace jbppo {
 
-constexpr int MAX_A = 8;
+constexpr int MAX_A = 8;        // continuous PPO, and every action count of the persistent kernel (ppo_fused.cu)
+constexpr int MAX_A_DISC = 18;  // discrete PPO row kernels (ppo.cu): ALE's full action set
 constexpr float F32_EPS = 1.1920928955078125e-07f;   // torch.finfo(float32).eps
 
 struct HP { float eps_clip, vf_coef, ent_coef; };
 
-struct RowOut {
-  float dpol[2 * MAX_A];   // d loss / d policy head outputs: discrete [A] logits; continuous [A] mu then [A] log_std
+// Register width of the per-action arrays of row<., NA>: MAX_A up to NA = 8, so those instantiations keep the layout the
+// persistent kernel is tuned for; NA itself above that.
+template <int NA> constexpr int width() { return NA > MAX_A ? NA : MAX_A; }
+
+template <int W = MAX_A>
+struct RowOutW {
+  float dpol[2 * W];       // d loss / d policy head outputs: discrete [A] logits; continuous [A] mu then [A] log_std
   float dv1, dv2;          // value-head gradient if critic_loss1 / critic_loss2 is the max (already x vf_coef / B)
   float sq1, sq2;          // (v - ret)^2, (v_clip - ret)^2
   float surr_min, ent;     // min(surr1, surr2), entropy (continuous: summed over dims)
   float ratio, pmin;       // ratio; exp(log_prob) (continuous: min over dims)
 };
+using RowOut = RowOutW<MAX_A>;
 
-// All per-action loops run over the compile-time bound MAX_A with an `a < A` guard: arrays stay in
-// registers (a run-time trip count would index them dynamically and put them in local memory) and the
-// arithmetic order is the plain ascending-a order of the restated definitions.
-template <int NA = MAX_A>
-__device__ __forceinline__ void log_softmax_row(const float (&lg)[MAX_A], int A, float (&lsm)[MAX_A]) {
+// All per-action loops run over a compile-time bound (NA, or the array width W >= NA) with an `a < A` guard: arrays stay
+// in registers (a run-time trip count would index them dynamically and put them in local memory) and the arithmetic
+// order is the plain ascending-a order of the restated definitions.
+template <int NA = MAX_A, int W>
+__device__ __forceinline__ void log_softmax_row(const float (&lg)[W], int A, float (&lsm)[W]) {
   float mx = lg[0];
 #pragma unroll
   for (int a = 1; a < NA; ++a) if (a < A) mx = fmaxf(mx, lg[a]);
@@ -35,7 +42,7 @@ __device__ __forceinline__ void log_softmax_row(const float (&lg)[MAX_A], int A,
   for (int a = 0; a < NA; ++a) if (a < A) s += expf(lg[a] - mx);
   const float ls = logf(s);
 #pragma unroll
-  for (int a = NA; a < MAX_A; ++a) lsm[a] = 0.f;
+  for (int a = NA; a < W; ++a) lsm[a] = 0.f;
 #pragma unroll
   for (int a = 0; a < NA; ++a) lsm[a] = a < A ? (lg[a] - mx) - ls : 0.f;
 }
@@ -58,10 +65,12 @@ __device__ __forceinline__ void surrogate(float ratio, float adv, float eps, flo
 
 // o: the row's head outputs [nout] (at least 2*MAX_A... entries readable up to index nout-1); a_disc / a_cont:
 // the stored action; lpo: log_prob_old (1 or A values)
-// NA: compile-time bound on A (the loops run to NA, guarded by a < A): row<., 2> costs a quarter of row<., 8>
-template <bool CONT, int NA = MAX_A>
+// NA: compile-time bound on A (the loops run to NA, guarded by a < A): row<., 2> costs a quarter of row<., 8>.
+// Continuous rows take NA <= MAX_A, discrete rows NA <= MAX_A_DISC.
+template <bool CONT, int NA = MAX_A, int W = width<NA>()>
 __device__ __forceinline__ void row(const float* o, int A, int a_disc, const float* a_cont, float adv, float ret,
-                                    float vold, const float* lpo, HP hp, float invB, RowOut& r) {
+                                    float vold, const float* lpo, HP hp, float invB, RowOutW<W>& r) {
+  static_assert(NA <= (CONT ? MAX_A : MAX_A_DISC) && W >= NA, "row: action bound out of range");
   float v = 0.f;                                   // o[CONT ? 2A : A] without a run-time register index
 #pragma unroll
   for (int q = 0; q < 2 * NA + 1; ++q) if (q == (CONT ? 2 * A : A)) v = o[q];
@@ -73,11 +82,11 @@ __device__ __forceinline__ void row(const float* o, int A, int a_disc, const flo
   r.dv1 = hp.vf_coef * invB * 2.f * d1;
   r.dv2 = hp.vf_coef * invB * 2.f * d2 * in_clip;
 #pragma unroll
-  for (int q = 0; q < 2 * MAX_A; ++q) r.dpol[q] = 0.f;
+  for (int q = 0; q < 2 * W; ++q) r.dpol[q] = 0.f;
   if (!CONT) {
-    float lg[MAX_A], lsm[MAX_A], pi[MAX_A], p[MAX_A], lc[MAX_A], inr[MAX_A];
+    float lg[W], lsm[W], pi[W], p[W], lc[W], inr[W];
 #pragma unroll
-    for (int a = 0; a < MAX_A; ++a) lg[a] = (a < NA && a < A) ? o[a] : 0.f;
+    for (int a = 0; a < W; ++a) lg[a] = (a < NA && a < A) ? o[a] : 0.f;
     log_softmax_row<NA>(lg, A, lsm);
     float S = 0.f;
 #pragma unroll
@@ -101,7 +110,7 @@ __device__ __forceinline__ void row(const float* o, int A, int a_disc, const flo
     r.surr_min = smin; r.ent = ent; r.ratio = ratio; r.pmin = expf(logp);
     const float dlogp = -gr * ratio * invB;            // d(actor_loss)/d log_prob
     const float dent = -hp.ent_coef * invB;            // d(ent_coef * entropy_loss)/d entropy_b
-    float dp[MAX_A], dot = 0.f;
+    float dp[W], dot = 0.f;
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
       dp[a] = 0.f;
@@ -112,7 +121,7 @@ __device__ __forceinline__ void row(const float* o, int A, int a_disc, const flo
         dot += t * pi[a];
       }
     }
-    float dlsm[MAX_A], sum_dlsm = 0.f;
+    float dlsm[W], sum_dlsm = 0.f;
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
       dlsm[a] = 0.f;
@@ -127,7 +136,7 @@ __device__ __forceinline__ void row(const float* o, int A, int a_disc, const flo
   } else {
     const float log_sqrt_2pi = 0.9189385332046727f;
     float dsum = 0.f, ent = 0.f;
-    float omu[MAX_A], ols[MAX_A], mu[MAX_A], sd[MAX_A], ls[MAX_A], z[MAX_A], dmu_[MAX_A], dls_[MAX_A];
+    float omu[W], ols[W], mu[W], sd[W], ls[W], z[W], dmu_[W], dls_[W];
 #pragma unroll
     for (int a = 0; a < NA; ++a) {                 // o[a] and o[A + a] without run-time register indices
       omu[a] = a < A ? o[a] : 0.f;

@@ -1,7 +1,8 @@
 """Throughput and memory of PPO on Atari frames (FrameRollout: states kept as single-frame references, conv1's im2col
 read from the frame ring), on one GPU, in one process:
 
-  reference   config.ppo.atari at the reference's scale: 8 envs, T=128, B=256 (distributed_batch_size), 3 epochs, H=512, A=4
+  reference   config.ppo.atari at the reference's scale: 8 envs, T=128, B=256 (distributed_batch_size), 3 epochs, H=512, on
+              --game (default breakout, A=4; seaquest has ALE's full 18 actions)
   scaled      the same with 1024 envs
 
 Each configuration runs one collect() + learn_rollout() as warm-up (CUDA-graph capture), then times three repeats of
@@ -10,7 +11,7 @@ learn_rollout() on the frame rollout and _learn_tensors() on the same rollout ma
 alternating 3x.  Also printed: the rollout's bytes per env (arithmetic) and the GPU's name, power limit and SM clock
 (read-only nvidia-smi query).
 
-  python scripts/ppo_frames_throughput.py [--repeats 3]
+  python scripts/ppo_frames_throughput.py [--repeats 3] [--game breakout]
 """
 import argparse
 import json
@@ -22,7 +23,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 from frame_replay_capacity import gpu_info  # noqa: E402
 
-T, B, EPOCHS, H, A = 128, 256, 3, 512, 4
+T, B, EPOCHS, H = 128, 256, 3, 512
+GAME = "breakout"
 FRAME = 84 * 84
 
 
@@ -38,9 +40,10 @@ def rollout_bytes_per_env(T):
 
 def _agent(n_step=T):
     from jorldy_b200.core import Agent
-    return Agent("ppo", state_size=[4, 84, 84], action_size=A, hidden_size=H, head="cnn", n_step=n_step, batch_size=B,
-                 n_epoch=EPOCHS, optim_config={"name": "adam", "lr": 2.5e-4}, run_step=10 ** 9, lr_decay=False,
-                 device="cuda")
+    from jorldy_b200.core.env.frames import _ACTIONS
+    return Agent("ppo", state_size=[4, 84, 84], action_size=_ACTIONS[GAME], hidden_size=H, head="cnn", n_step=n_step,
+                 batch_size=B, n_epoch=EPOCHS, optim_config={"name": "adam", "lr": 2.5e-4}, run_step=10 ** 9,
+                 lr_decay=False, device="cuda")
 
 
 def _timed(fn):
@@ -60,7 +63,7 @@ def run_config(name, N, repeats):
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
     agent = _agent()
-    col = RolloutCollector(Env("breakout", num_envs=N, seed=0, device="cuda"), agent)
+    col = RolloutCollector(Env(GAME, num_envs=N, seed=0, device="cuda"), agent)
     agent.learn_rollout(col.collect())                  # warm-up: graph capture of collect and of the minibatch chunk
     torch.cuda.synchronize()
     tc, tl = [], []
@@ -70,7 +73,8 @@ def run_config(name, N, repeats):
         tc.append(c_ms)
         tl.append(l_ms)
     tot = [c + l for c, l in zip(tc, tl)]
-    out = {"config": name, "envs": N, "T": T, "batch_size": B, "n_epoch": EPOCHS, "hidden": H, "actions": A,
+    out = {"config": name, "envs": N, "T": T, "batch_size": B, "n_epoch": EPOCHS, "hidden": H, "game": GAME,
+           "actions": agent.action_size,
            "env_steps_per_sec": N * T / (min(tot) / 1e3),
            "learner_transitions_per_sec": N * T * EPOCHS / (min(tl) / 1e3),
            "ms_collect_best": min(tc), "ms_collect_spread": max(tc) - min(tc),
@@ -90,7 +94,7 @@ def compare(N, repeats):
     torch.cuda.empty_cache()
     a, b = _agent(), _agent()
     b.network.load_state_dict(a.network.state_dict())
-    ro = RolloutCollector(Env("breakout", num_envs=N, seed=0, device="cuda"), a).collect()
+    ro = RolloutCollector(Env(GAME, num_envs=N, seed=0, device="cuda"), a).collect()
     refs = ro.state_ref.reshape(-1)
     stacks, _ = ro.frames.gather(refs, refs)
     last, _ = ro.frames.gather(ro.last_next_state, ro.last_next_state)
@@ -120,7 +124,10 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--scaled-envs", type=int, default=1024)
     ap.add_argument("--compare-envs", type=int, default=256)
+    ap.add_argument("--game", type=str, default="breakout")
     args = ap.parse_args()
+    global GAME
+    GAME = args.game
     import torch
     if not torch.cuda.is_available():
         sys.exit("ppo_frames_throughput.py measures on a CUDA device; none is available")
