@@ -70,7 +70,7 @@ constexpr int RED_FLOATS = KG * (32 * 36 + 16);   /* = KG * RED_GS */         //
 constexpr int JA_ROWS = 256;                            // minibatch rows per dW2 / head-gradient panel
 constexpr int R2_FLOATS = JA_ROWS * 32;                 // 8192: a dense [256][32] panel
 constexpr int MAX_B = 512;                              // minibatch rows (row-phase scratch in s_small)
-constexpr int ADAM_IT = 8;                              // float4 per thread kept in registers across the barrier
+constexpr int ADAM_IT = 4;                              // float4 per thread kept in registers across the barrier
 constexpr int PS_FLOATS = (MAXO + 2) * PK;                // per-CTA parameter stash: head rows [MAXO][PK], b2, b1
 constexpr int CTR_JB = 32;                              // a.barrier[CTR_JB + kt]: finished JB jobs of column tile kt
 
@@ -1527,7 +1527,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           shadow(i, pp[it]);
         }
       }
-      for (long long i = lo + tid + (long long)ADAM_IT * NT; i < hi; i += NT) {   // slices beyond 8 K floats per CTA
+      for (long long i = lo + tid + (long long)ADAM_IT * NT; i < hi; i += NT) {   // slices beyond 4 K floats per CTA
         float4 p_ = __ldcg(p4 + i), m_ = __ldcg(m4 + i), v_ = __ldcg(v4 + i);
         float4 g_;
         if (a.world > 1) {

@@ -1,16 +1,33 @@
-"""Intra-step timeline of the persistent PPO kernel: clock64 stamps of the last step (debug trace, JB_FUSED_SKIP=256)."""
-import sys, os, ctypes
-os.environ["JB_FUSED_SKIP"] = "256"
+"""Intra-step timeline of the persistent PPO kernel: clock64 stamps of the last step (debug trace, JB_FUSED_SKIP=256).
+
+    python scripts/perf_trace.py [--config cartpole|continuous] [--batch B] --ghz F
+
+--config cartpole: D=4, A=2 discrete (bench ppo_cartpole, B=256); continuous: D=11, A=3 Gaussian (bench ppo_continuous,
+B=512).  --ghz converts clock64 ticks to microseconds: pass the SM clock the card actually ran at
+(`nvidia-smi --query-gpu=clocks.max.sm`), it is not read here."""
+import argparse, ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--config", choices=("cartpole", "continuous"), default="cartpole")
+ap.add_argument("--batch", type=int, default=None)
+ap.add_argument("--ghz", type=float, required=True)
+args = ap.parse_args()
+os.environ["JB_FUSED_SKIP"] = "256"
+
 import numpy as np, torch
 from jorldy_b200.core import Agent, Env
 from jorldy_b200.core.collect import RolloutCollector
 from jorldy_b200._lib import C
 
-N, T, B = 4096, 32, int(os.environ.get("B", 256))
-env = Env("cartpole", num_envs=N, seed=0)
-agent = Agent("ppo", state_size=4, action_size=2, hidden_size=512, batch_size=B, n_step=T, n_epoch=1,
-              optim_config={"name": "adam", "lr": 2.5e-4}, device="cuda", run_step=10**9, use_fused=True)
+if args.config == "cartpole":
+    env_name, D, A, kw, B = "cartpole", 4, 2, {}, args.batch or 256
+else:
+    env_name, D, A, kw, B = "hopper", 11, 3, {"network": "continuous_policy_value"}, args.batch or 512
+N, T = 4096, 32
+env = Env(env_name, num_envs=N, seed=0)
+agent = Agent("ppo", state_size=D, action_size=A, hidden_size=512, batch_size=B, n_step=T, n_epoch=1,
+              optim_config={"name": "adam", "lr": 2.5e-4}, device="cuda", run_step=10**9, use_fused=True, **kw)
 col = RolloutCollector(env, agent, use_cuda_graph=False); col.collect()
 agent.learn_rollout(col.rollout); col.rollout.t = T
 st = agent._st; fr = agent._fused[B]
@@ -18,7 +35,7 @@ n = N * T // B
 torch.cuda.synchronize()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 agent._cursor.zero_(); e0.record(); fr.run(st, n); e1.record(); torch.cuda.synchronize()
-print(f"{e0.elapsed_time(e1)/n*1000:.1f} us/step over {n} steps")
+print(f"{args.config} B={B}: {e0.elapsed_time(e1)/n*1000:.1f} us/step over {n} steps (traced)")
 tr = np.zeros((256, 48), np.int64)
 C.jb_ppo_fused_trace(tr.ctypes.data_as(ctypes.c_void_p))
 names = {0: "step start", 1: "P1 h1 generated", 2: "P1 panel landed", 3: "P1 mma", 4: "P1 reduce", 5: "P1 end", 6: "bar1",
@@ -27,7 +44,7 @@ names = {0: "step start", 1: "P1 h1 generated", 2: "P1 panel landed", 3: "P1 mma
          17: "JA staged", 18: "JA dh2 gen", 19: "JA mma(last)", 20: "JA reduce(last)", 21: "JA end",
          22: "P3 jobs end", 28: "P1 stash issued", 29: "P1 stash landed", 31: "row: head outputs", 32: "row: math done",
          33: "JB dW1 staged", 34: "JB dW1 stored", 35: "P1 shuffles done", 36: "row: perm issued", 23: "norm partial + p/m/v issued", 24: "bar3", 25: "P5 fold", 26: "P5 end", 27: "bar5"}
-ghz = 1.98                                  # H100 SXM boost clock (clock64 ticks -> us)
+ghz = args.ghz
 n = int((tr[:, 0] > 0).sum())               # CTAs of the launch
 for cta in sorted({0, n // 2, n - 1}):
     t = tr[cta]
@@ -35,7 +52,7 @@ for cta in sorted({0, n // 2, n - 1}):
     order = sorted([i for i in names if t[i] > 0], key=lambda i: t[i])
     prev = t[0]
     for i in order:
-        print(f"  {names[i]:22s} +{(t[i]-prev)/ghz/1000:6.2f} us   @{(t[i]-t[0])/ghz/1000:6.2f}")
+        print(f"  {names[i]:28s} +{(t[i]-prev)/ghz/1000:6.2f} us   @{(t[i]-t[0])/ghz/1000:6.2f}")
         prev = t[i]
 # barrier waits: arrival spread
 for a_, b_, nm in [(5, 6, "bar1"), (23, 24, "bar3"), (26, 27, "bar5")]:
