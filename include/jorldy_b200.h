@@ -294,4 +294,34 @@ JB_API int jb_sacd_critic_loss(const float* q1, const float* q2, const float* nq
 JB_API int jb_sacd_actor(const float* logits, const float* q1, const float* q2, const float* alpha, float target_entropy,
                          int B, int A, float* dlogits, float* stats4, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Quantile regression (QR-DQN arXiv:1710.10044, IQN arXiv:1806.06923), csrc/quantile.cu.
+ * A quantile tensor holds A actions x N quantiles per sample at offset b*A*N + a*sa + i*sq:
+ * [B, A, K] is (sa, sq) = (K, 1), [B, N, A] is (1, A).
+ *   jb_quantile_loss   y_j = r + ((1-d) gamma) next_target[b, a*, j], a* = argmax_a mean_j next_target[b, a, j];
+ *                      u_ij = y_j - pred[b, a_b, i], rho = |tau_i - 1{u < 0}| smooth_l1(u), tau_i = tau[b*tau_stride + i]
+ *                      (tau_stride 0: one shared set of fractions);
+ *                      loss[b] = (1/Np) sum_j sum_i rho_ij, dpred[b, a_b, i] = -(1/(B Np)) sum_j |tau_i - 1{u<0}| clamp(u,-1,1),
+ *                      0 on every other action; a_star [B] (may be NULL); stats = {mean_b loss[b], max_{b,a} mean_i pred};
+ *                      scratch: 2*B floats.  1 <= A <= 18, 1 <= N, Np <= 256, else JB_ERR_INVALID.  One CTA per sample,
+ *                      fixed-order sums: bit-reproducible.
+ *   jb_quantile_mean   q [M, A] = mean over the N quantiles of x (same layout convention)
+ *   jb_iqn_tau         tau [rows, N] ~ U[lo, hi) from Philox(seed, stream_id, ctr[0] + e/4) word e%4; ctr[0] += ceil(rows*N/4)
+ *   jb_iqn_cos         c [rows, E] = cos(pi i tau[r]), i < E
+ *   jb_iqn_mul_fwd     z [B, N, D] = psi [B, D] (*) phi [B, N, D]
+ *   jb_iqn_mul_bwd     dpsi [B, D] = 1{psi > 0} sum_n dz (*) phi (n ascending; psi is the head's ReLU output, so this is
+ *                      the gradient w.r.t. its pre-activation), dpre [B, N, D] = dz (*) psi (*) 1{phi > 0}
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_quantile_loss(const float* pred, int p_sa, int p_sq, const float* next_target, int t_sa, int t_sq,
+                            const float* tau, int tau_stride, const void* action, int action_kind, const float* reward,
+                            const float* done, int B, int A, int N, int Np, float gamma, float* dpred, float* loss,
+                            int32_t* a_star, float* stats, float* scratch, void* stream);
+JB_API int jb_quantile_mean(const float* x, int sa, int sq, int M, int A, int N, float* q, void* stream);
+JB_API int jb_iqn_tau(float* tau, int rows, int N, float lo, float hi, uint64_t seed, uint64_t stream_id, long long* ctr,
+                      void* stream);
+JB_API int jb_iqn_cos(const float* tau, int rows, int E, float* c, void* stream);
+JB_API int jb_iqn_mul_fwd(const float* psi, const float* phi, int B, int N, int D, float* z, void* stream);
+JB_API int jb_iqn_mul_bwd(const float* dz, const float* psi, const float* phi, int B, int N, int D, float* dpsi, float* dpre,
+                          void* stream);
+
 #endif /* JORLDY_B200_H */

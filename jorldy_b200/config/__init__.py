@@ -3,7 +3,7 @@
 `load("config.<agent>.<env>")` returns a module-like namespace with the four dicts the reference's
 config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / train).  Values follow the
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
-per, noisy, c51, rainbow, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar / pendulum / atari(synthetic) /
+per, noisy, c51, rainbow, qrdqn, iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar / pendulum / atari(synthetic) /
 mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
@@ -31,6 +31,9 @@ _VALUE_AGENTS = {
     "c51": ("discrete_q_network", dict(_EPS, v_min=-1, v_max=10, num_support=51), 5, 32),
     "rainbow": ("rainbow", dict(n_step=3, alpha=0.5, beta=0.4, learn_period=2, uniform_sample_prob=1e-3,
                                 noise_type="factorized", v_min=-1, v_max=10, num_support=51), 10, 8),
+    # quantile agents (arXiv:1710.10044, arXiv:1806.06923): DQN's keys plus the papers' quantile counts
+    "qrdqn": ("discrete_q_network", dict(_EPS, num_support=200), 10, 32),
+    "iqn": ("iqn", dict(_EPS, num_sample=64, embedding_dim=64, sample_min=0.0, sample_max=1.0), 10, 32),
 }
 
 

@@ -4,9 +4,10 @@ from collections import OrderedDict
 from .ppo import PPO
 from .dqn import DQN, Double, Dueling, Multistep, PER, Noisy, C51, Rainbow, ApeX
 from .ddpg import DDPG, TD3, SAC
+from .quantile import IQN, QRDQN
 
-agent_dict = OrderedDict(sorted(dict(ape_x=ApeX, c51=C51, ddpg=DDPG, double=Double, dqn=DQN, dueling=Dueling,
-                                     multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, rainbow=Rainbow, sac=SAC,
+agent_dict = OrderedDict(sorted(dict(ape_x=ApeX, c51=C51, ddpg=DDPG, double=Double, dqn=DQN, dueling=Dueling, iqn=IQN,
+                                     multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, qrdqn=QRDQN, rainbow=Rainbow, sac=SAC,
                                      td3=TD3).items()))
 
 

@@ -4,6 +4,7 @@ from collections import OrderedDict
 
 from .policy_value import DiscretePolicyValue, ContinuousPolicyValue, DiscreteQ_Network
 from .dueling import Dueling
+from .iqn import IQN
 from .noisy import Noisy, Rainbow
 from .policy import ContinuousPolicy, DeterministicPolicy, DiscretePolicy
 from .q_network import ContinuousQ_Network
@@ -17,6 +18,7 @@ network_dict = OrderedDict(
     discrete_policy_value=DiscretePolicyValue,
     discrete_q_network=DiscreteQ_Network,
     dueling=Dueling,
+    iqn=IQN,
     noisy=Noisy,
     rainbow=Rainbow,
 )
