@@ -470,7 +470,8 @@ JB_API int jb_sac_minq(const float* q1, const float* q2, const float* logp, cons
 
 JB_API int jb_sac_actor_bwd(const float* raw, int nout, const float* eps, const float* action, const float* da,
                             const float* alpha, int B, int A, float* dout, void* stream) {
-  if (!raw || !eps || !action || !da || !alpha || !dout || B <= 0 || A <= 0 || nout != 2 * A) return JB_ERR_INVALID;
+  if (!raw || !eps || !action || !da || !alpha || !dout || B <= 0 || A <= 0 || A > AC_MAX_A || nout != 2 * A)
+    return JB_ERR_INVALID;
   sac_actor_bwd_kernel<<<jb_div_up((long long)B * A, 256), 256, 0, (cudaStream_t)stream>>>(raw, nout, eps, action, da, alpha, B, A, dout);
   return jb_check_launch();
 }
