@@ -324,4 +324,33 @@ JB_API int jb_iqn_mul_fwd(const float* psi, const float* phi, int B, int N, int 
 JB_API int jb_iqn_mul_bwd(const float* dz, const float* psi, const float* phi, int B, int N, int D, float* dpsi, float* dpre,
                           void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Munchausen RL (M-DQN, M-IQN; Vieillard, Pietquin, Geist 2020, arXiv:2007.14430), csrc/munchausen.cuh with
+ * csrc/dqn.cu and csrc/quantile.cu.  q'(s, .) and q'(s', .) are the TARGET network's Q; tau is the entropy temperature
+ * (m_tau), alpha the Munchausen scale (m_alpha), l0 the clip floor.  Per sample, one thread, actions ascending:
+ *   tau logpi(a|s)  = (q'(s,a) - m) - tau log sum_b exp((q'(s,b) - m)/tau),  m = max_b q'(s,b)   (log(pi) is never formed)
+ *   pi'(a)          = softmax(q'(s',.)/tau)(a),  tau logpi'(a|s') in the same stable form
+ *   bonus           = alpha clip(tau logpi(a_t|s), l0, 0)        (clipped first, then scaled)
+ *   jb_mdqn_loss    y = r + bonus + ((1-d) gamma) sum_a pi'(a) (qt_next[b,a] - tau logpi'(a|s')), q' = qt_s / qt_next [B, A];
+ *                   loss = mean_b smooth_l1(q[b, a_b] - y), dq[b, a_b] = smooth_l1'(q - y)/B, 0 on every other action;
+ *                   stats = {loss, max_b q[b, a_b]}; reward / done [B]; scratch: 2*B floats.  One warp per sample.
+ *   jb_munchausen_quantile_loss
+ *                   [B, N, A] layout only (pred, next_target [B, Np, A], cur_target [B, Nc, A]); q'(s, .) and q'(s', .)
+ *                   are the means over cur_target's Nc and next_target's Np quantiles;
+ *                   y_j = r + bonus + ((1-d) gamma) sum_a pi'(a) (next_target[b, j, a] - tau logpi'(a|s'));
+ *                   the loss and dpred are jb_quantile_loss's quantile Huber (kappa = 1) on these y_j with the
+ *                   fractions tau[b*tau_stride + i]; stats = {mean_b loss[b], max_{b,a} mean_i pred}; scratch: 2*B floats.
+ *                   One CTA per sample.
+ * Both: 1 <= A <= 18, 1 <= N, Np, Nc <= 256, m_tau > 0, l0 <= 0, else JB_ERR_INVALID.  Fixed-order sums and a single-thread
+ * finalize, no atomics: bit-reproducible.  At m_alpha = 0 with m_tau -> 0 and a unique argmax, pi' is one-hot and both
+ * reduce to jb_td_loss (order 0) and jb_quantile_loss.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_mdqn_loss(const float* q, const float* qt_s, const float* qt_next, const void* action, int action_kind,
+                        const float* reward, const float* done, int B, int A, float gamma, float m_alpha, float m_tau,
+                        float l0, float* dq, float* stats, float* scratch, void* stream);
+JB_API int jb_munchausen_quantile_loss(const float* pred, const float* next_target, const float* cur_target, const float* tau,
+                                       int tau_stride, const void* action, int action_kind, const float* reward,
+                                       const float* done, int B, int A, int N, int Np, int Nc, float gamma, float m_alpha,
+                                       float m_tau, float l0, float* dpred, float* stats, float* scratch, void* stream);
+
 #endif /* JORLDY_B200_H */

@@ -3,8 +3,8 @@
 `load("config.<agent>.<env>")` returns a module-like namespace with the four dicts the reference's
 config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / train).  Values follow the
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
-per, noisy, c51, rainbow, qrdqn, iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar / pendulum / atari(synthetic) /
-mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
+per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
+pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
@@ -34,6 +34,10 @@ _VALUE_AGENTS = {
     # quantile agents (arXiv:1710.10044, arXiv:1806.06923): DQN's keys plus the papers' quantile counts
     "qrdqn": ("discrete_q_network", dict(_EPS, num_support=200), 10, 32),
     "iqn": ("iqn", dict(_EPS, num_sample=64, embedding_dim=64, sample_min=0.0, sample_max=1.0), 10, 32),
+    # Munchausen agents (arXiv:2007.14430): DQN's / IQN's rows plus the paper's alpha, tau and l_0
+    "m_dqn": ("discrete_q_network", dict(_EPS, alpha=0.9, tau=0.03, l_0=-1), 10, 32),
+    "m_iqn": ("iqn", dict(_EPS, num_sample=64, embedding_dim=64, sample_min=0.0, sample_max=1.0, alpha=0.9, tau=0.03, l_0=-1),
+              10, 32),
 }
 
 

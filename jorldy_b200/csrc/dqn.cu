@@ -12,6 +12,7 @@
 // `.item()` device->host syncs to write priorities one by one; here it is one launch, with the
 // new priorities left in device memory (f64, as the sum-tree wants them).
 #include "common.cuh"
+#include "munchausen.cuh"
 #include "philox.cuh"
 
 namespace {
@@ -153,6 +154,47 @@ td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, co
   }
 }
 
+// ---- Munchausen DQN loss (arXiv:2007.14430) ------------------------------------------------------
+// One warp per sample; lane 0 forms the target in a fixed order (munchausen.cuh), the warp writes the sample's dq row.
+// The per-sample loss and Q(s)[a_t] go to partial[2b], partial[2b + 1] and one thread folds them (mdqn_finalize_kernel).
+constexpr int MDQN_WARPS = 4;
+
+__global__ void __launch_bounds__(MDQN_WARPS * 32)
+mdqn_loss_kernel(const float* __restrict__ q, const float* __restrict__ qt_s, const float* __restrict__ qt_next,
+                 const void* __restrict__ action, int action_kind, const float* __restrict__ reward,
+                 const float* __restrict__ done, int B, int A, float gamma, float m_alpha, float m_tau, float l0,
+                 float* __restrict__ dq, float* __restrict__ partial /*[B][2]*/) {
+  __shared__ float s_pi[MDQN_WARPS][MUNCHAUSEN_MAX_A], s_tlp[MDQN_WARPS][MUNCHAUSEN_MAX_A];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x * MDQN_WARPS + warp;
+  if (b >= B) return;
+  const int a_t = read_action(action, action_kind, b);
+  float g = 0.f;
+  if (lane == 0) {
+    const float* qn = qt_next + (size_t)b * A;
+    const float bonus = munchausen_row(qt_s + (size_t)b * A, qn, A, a_t, m_tau, m_alpha, l0, s_pi[warp], s_tlp[warp]);
+    float v = 0.f;
+    for (int a = 0; a < A; ++a) v += s_pi[warp][a] * (qn[a] - s_tlp[warp][a]);
+    const float nd = __fmul_rn(__fadd_rn(1.f, -done[b]), gamma);
+    const float y = __fadd_rn(__fadd_rn(reward[b], bonus), __fmul_rn(nd, v));
+    const float q_b = q[(size_t)b * A + a_t];
+    const float diff = q_b - y, ad = fabsf(diff);                 // F.smooth_l1_loss(q, y), beta = 1, as td_loss_kernel
+    g = ad < 1.f ? diff : (diff > 0.f ? 1.f : -1.f);
+    partial[2 * b] = ad < 1.f ? 0.5f * diff * diff : ad - 0.5f;
+    partial[2 * b + 1] = q_b;
+  }
+  g = __shfl_sync(0xffffffffu, g, 0) / (float)B;
+  for (int a = lane; a < A; a += 32) dq[(size_t)b * A + a] = a == a_t ? g : 0.f;
+}
+
+__global__ void mdqn_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
+  if (threadIdx.x != 0) return;
+  float l = 0.f, mq = -INFINITY;
+  for (int b = 0; b < B; ++b) { l += partial[2 * b]; mq = fmaxf(mq, partial[2 * b + 1]); }
+  stats[0] = l / (float)B;   // loss
+  stats[1] = mq;             // max_Q = max over the batch of Q(s)[a], as td_loss_kernel
+}
+
 }  // namespace
 
 JB_API int jb_q_act(const float* q, int M, int A, float eps, const float* eps_rows, const float* u, uint64_t seed,
@@ -188,5 +230,21 @@ JB_API int jb_td_loss(const float* q, const float* q_next, const float* qt_next,
   const int threads = ((B + 31) / 32) * 32;
   td_loss_kernel<<<1, threads, 0, (cudaStream_t)stream>>>(q, q_next, qt_next, action, action_kind, reward, done, weights,
                                                          B, A, hp, dq, prio, stats);
+  return jb_check_launch();
+}
+
+// M-DQN: q[B,A] online Q(s); qt_s[B,A] target Q(s); qt_next[B,A] target Q(s'); reward/done [B] f32.
+// y = r + alpha clip(tau logpi(a|s), l0, 0) + ((1-d) gamma) sum_a pi'(a) (qt_next[a] - tau logpi'(a|s')) (munchausen.cuh);
+// dq[b, a_b] = smooth_l1'(q - y)/B, 0 elsewhere; stats[2] = {loss, max_Q}; scratch: 2*B floats.
+JB_API int jb_mdqn_loss(const float* q, const float* qt_s, const float* qt_next, const void* action, int action_kind,
+                        const float* reward, const float* done, int B, int A, float gamma, float m_alpha, float m_tau,
+                        float l0, float* dq, float* stats, float* scratch, void* stream) {
+  if (!q || !qt_s || !qt_next || !action || !reward || !done || !dq || !stats || !scratch) return JB_ERR_INVALID;
+  if (B <= 0 || A <= 0 || A > MUNCHAUSEN_MAX_A || action_kind < 0 || action_kind > 2 || !(m_tau > 0.f) || !(l0 <= 0.f))
+    return JB_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  mdqn_loss_kernel<<<jb_div_up(B, MDQN_WARPS), MDQN_WARPS * 32, 0, s>>>(q, qt_s, qt_next, action, action_kind, reward, done,
+                                                                       B, A, gamma, m_alpha, m_tau, l0, dq, scratch);
+  mdqn_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }

@@ -8,8 +8,10 @@
 //   rho_ij = |tau_i - 1{u_ij < 0}| h(u_ij),  h = smooth_l1,  loss = (1/B) sum_b (1/N') sum_j sum_i rho_ij
 //   d loss / d theta_i = -(1/(B N')) sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -1, 1)  (0 on non-taken actions)
 // a* = argmax_a mean_j theta'_j(s', a), first index on ties.  Every sum runs in a fixed order (no atomics), and the
-// batch statistics are folded by one thread, so a learn() is bit-reproducible.
+// batch statistics are folded by one thread, so a learn() is bit-reproducible.  M-IQN's loss (arXiv:2007.14430) runs the
+// same per-sample Huber loop on Munchausen targets (munchausen.cuh).
 #include "common.cuh"
+#include "munchausen.cuh"
 #include "philox.cuh"
 
 namespace {
@@ -17,6 +19,7 @@ namespace {
 constexpr int QMAXN = 256;     // quantiles per pass (N, N')
 constexpr int QMAXA = 18;      // ALE's full action set
 constexpr int QT = 256;        // threads per CTA of the loss kernel: one predicted quantile each
+static_assert(QMAXA == MUNCHAUSEN_MAX_A, "M-IQN's pi' / tau logpi' rows hold every action");
 
 __device__ __forceinline__ int read_action(const void* act, int kind, int b) {
   if (kind == 0) return (int)((const int64_t*)act)[b];
@@ -30,6 +33,39 @@ __device__ __forceinline__ float warp_mean(const float* __restrict__ x, int sq, 
   float s = 0.f;
   for (int j = lane; j < n; j += 32) s += x[(size_t)j * sq];
   return jb_warp_sum(s) / (float)n;
+}
+
+// The quantile Huber loss of one sample, given its targets s_y[0, Np) and fractions s_tau[0, N) in shared memory: thread
+// i < N owns predicted quantile i of the taken action a_t and sums over j in order.  Writes the sample's dpred row db (0 on
+// every other action) and returns (1/Np) sum_j sum_i rho_ij on thread 0 (a fixed-order tree over the warps).
+__device__ __forceinline__ float quantile_huber(const float* __restrict__ pb, int p_sa, int p_sq, const float* s_y,
+                                                const float* s_tau, float* s_red, int A, int N, int Np, int a_t, float gcoef,
+                                                float* __restrict__ db) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  float li = 0.f;
+  if (tid < N) {
+    const float th = pb[(size_t)a_t * p_sa + (size_t)tid * p_sq];
+    const float t = s_tau[tid], tc = 1.f - t;
+    float g = 0.f;
+    for (int j = 0; j < Np; ++j) {
+      const float u = s_y[j] - th, au = fabsf(u);
+      const float w = u < 0.f ? tc : t;
+      li += w * (au < 1.f ? 0.5f * u * u : au - 0.5f);
+      g += w * fminf(fmaxf(u, -1.f), 1.f);
+    }
+    db[(size_t)a_t * p_sa + (size_t)tid * p_sq] = -g * gcoef;
+  }
+  for (int e = tid; e < A * N; e += QT) {
+    const int a = e / N, i = e - a * N;
+    if (a != a_t) db[(size_t)a * p_sa + (size_t)i * p_sq] = 0.f;
+  }
+  li = jb_warp_sum(li);
+  if (lane == 0) s_red[warp] = li;
+  __syncthreads();
+  float s = 0.f;
+  if (tid == 0)
+    for (int w = 0; w < QT / 32; ++w) s += s_red[w];
+  return s / (float)Np;
 }
 
 __global__ void __launch_bounds__(QT)
@@ -59,32 +95,54 @@ quantile_loss_kernel(const float* __restrict__ pred, int p_sa, int p_sq, const f
   for (int j = tid; j < Np; j += QT) s_y[j] = __fadd_rn(r, __fmul_rn(nd, tb[(size_t)a_star * t_sa + (size_t)j * t_sq]));
   const int a_t = read_action(action, action_kind, b);
   __syncthreads();
-  float li = 0.f;
-  if (tid < N) {
-    const float th = pb[(size_t)a_t * p_sa + (size_t)tid * p_sq];
-    const float t = s_tau[tid], tc = 1.f - t;
-    float g = 0.f;
-    for (int j = 0; j < Np; ++j) {
-      const float u = s_y[j] - th, au = fabsf(u);
-      const float w = u < 0.f ? tc : t;
-      li += w * (au < 1.f ? 0.5f * u * u : au - 0.5f);
-      g += w * fminf(fmaxf(u, -1.f), 1.f);
-    }
-    dpred[(size_t)b * A * N + (size_t)a_t * p_sa + (size_t)tid * p_sq] = -g * gcoef;
-  }
-  for (int e = tid; e < A * N; e += QT) {
-    const int a = e / N, i = e - a * N;
-    if (a != a_t) dpred[(size_t)b * A * N + (size_t)a * p_sa + (size_t)i * p_sq] = 0.f;
-  }
-  li = jb_warp_sum(li);
-  if (lane == 0) s_red[warp] = li;
-  __syncthreads();
+  const float lb = quantile_huber(pb, p_sa, p_sq, s_y, s_tau, s_red, A, N, Np, a_t, gcoef, dpred + (size_t)b * A * N);
   if (tid == 0) {
-    float s = 0.f;
-    for (int w = 0; w < QT / 32; ++w) s += s_red[w];
-    const float lb = s / (float)Np;
     loss_out[b] = lb;
     if (a_star_out) a_star_out[b] = a_star;
+    partial[2 * b] = lb;
+    partial[2 * b + 1] = maxq;
+  }
+}
+
+// M-IQN (arXiv:2007.14430) on the [B, N, A] layout: q'(s, .) and q'(s', .) are the per-action means of the target
+// network's quantiles on s (Nc fractions) and on s' (Np fractions); thread 0 forms the Munchausen scalars (munchausen.cuh)
+// and y_j = (r + bonus) + ((1 - d) gamma) sum_a pi'(a) (theta'_j(s', a) - tau logpi'(a|s')), actions ascending.  The loss is
+// quantile_huber's, unchanged.
+__global__ void __launch_bounds__(QT)
+munchausen_quantile_loss_kernel(const float* __restrict__ pred, const float* __restrict__ nxt, const float* __restrict__ cur,
+                                const float* __restrict__ tau, int tau_stride, const void* __restrict__ action,
+                                int action_kind, const float* __restrict__ reward, const float* __restrict__ done, int A,
+                                int N, int Np, int Nc, float gamma, float m_alpha, float m_tau, float l0, float gcoef,
+                                float* __restrict__ dpred, float* __restrict__ partial /*[B][2]*/) {
+  __shared__ float s_y[QMAXN], s_tau[QMAXN], s_q[3][QMAXA], s_pi[QMAXA], s_tlp[QMAXA], s_red[QT / 32], s_bonus;
+  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* pb = pred + (size_t)b * A * N;
+  const float* tb = nxt + (size_t)b * A * Np;
+  // s_q rows: the online mean on s (for max_Q), the target means on s' and on s
+  for (int e = warp; e < 3 * A; e += QT / 32) {
+    const int k = e / A, a = e - k * A;
+    const int n = k == 0 ? N : (k == 1 ? Np : Nc);
+    const float* x = k == 0 ? pb : (k == 1 ? tb : cur + (size_t)b * A * Nc);
+    const float v = warp_mean(x + a, A, n, lane);
+    if (lane == 0) s_q[k][a] = v;
+  }
+  for (int i = tid; i < N; i += QT) s_tau[i] = tau[(size_t)b * tau_stride + i];
+  const int a_t = read_action(action, action_kind, b);
+  __syncthreads();
+  if (tid == 0) s_bonus = munchausen_row(s_q[2], s_q[1], A, a_t, m_tau, m_alpha, l0, s_pi, s_tlp);
+  __syncthreads();
+  const float base = __fadd_rn(reward[b], s_bonus), nd = __fmul_rn(__fadd_rn(1.f, -done[b]), gamma);
+  for (int j = tid; j < Np; j += QT) {
+    const float* tj = tb + (size_t)j * A;
+    float v = 0.f;
+    for (int a = 0; a < A; ++a) v += s_pi[a] * (tj[a] - s_tlp[a]);
+    s_y[j] = __fadd_rn(base, __fmul_rn(nd, v));
+  }
+  __syncthreads();
+  const float lb = quantile_huber(pb, 1, A, s_y, s_tau, s_red, A, N, Np, a_t, gcoef, dpred + (size_t)b * A * N);
+  if (tid == 0) {
+    float maxq = s_q[0][0];
+    for (int a = 1; a < A; ++a) maxq = fmaxf(maxq, s_q[0][a]);
     partial[2 * b] = lb;
     partial[2 * b + 1] = maxq;
   }
@@ -123,6 +181,24 @@ JB_API int jb_quantile_loss(const float* pred, int p_sa, int p_sq, const float* 
   cudaStream_t s = (cudaStream_t)stream;
   quantile_loss_kernel<<<B, QT, 0, s>>>(pred, p_sa, p_sq, next_target, t_sa, t_sq, tau, tau_stride, action, action_kind,
                                         reward, done, A, N, Np, gamma, gcoef, dpred, loss, a_star, scratch);
+  quantile_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  return jb_check_launch();
+}
+
+JB_API int jb_munchausen_quantile_loss(const float* pred, const float* next_target, const float* cur_target, const float* tau,
+                                       int tau_stride, const void* action, int action_kind, const float* reward,
+                                       const float* done, int B, int A, int N, int Np, int Nc, float gamma, float m_alpha,
+                                       float m_tau, float l0, float* dpred, float* stats, float* scratch, void* stream) {
+  if (!pred || !next_target || !cur_target || !tau || !action || !reward || !done || !dpred || !stats || !scratch)
+    return JB_ERR_INVALID;
+  if (B <= 0 || A <= 0 || A > QMAXA || N <= 0 || N > QMAXN || Np <= 0 || Np > QMAXN || Nc <= 0 || Nc > QMAXN ||
+      tau_stride < 0 || action_kind < 0 || action_kind > 2 || !(m_tau > 0.f) || !(l0 <= 0.f))
+    return JB_ERR_INVALID;
+  const float gcoef = (float)(1.0 / ((double)B * (double)Np));
+  cudaStream_t s = (cudaStream_t)stream;
+  munchausen_quantile_loss_kernel<<<B, QT, 0, s>>>(pred, next_target, cur_target, tau, tau_stride, action, action_kind,
+                                                   reward, done, A, N, Np, Nc, gamma, m_alpha, m_tau, l0, gcoef, dpred,
+                                                   scratch);
   quantile_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }
