@@ -24,6 +24,9 @@ typedef struct jb_ppo_fused_args {
   float *xg;                         /* [B, D] */
   float *w1p;                        /* [B/32, H, D+1] per-row-tile partial dW1 | db1 */
   float *headp;                      /* [H/32, 2, B, 4] per-column-tile partial head outputs */
+  float *dout;                       /* [B, 8] d loss / d head outputs per row (value head: the critic_loss1 candidate) */
+  float *dv2;                        /* [B] the critic_loss2 candidate of the value-head gradient */
+  float *rowst;                      /* [6, B] per-row v - ret, v_clip - ret, min(surr1, surr2), entropy, ratio, p_min */
   float *h2t;                        /* [H/32, B, 32] tiled copy of h2 */
   float *W2t;                        /* [H/32, H, 32] tiled shadow of W2 (maintained by the Adam phase) */
   float *W2img;                      /* [2 (hi | lo), H/32, H/32, 32 x 32] wgmma-layout (K-major, 128-byte swizzle) images of W2 for the tensor-core
@@ -32,7 +35,7 @@ typedef struct jb_ppo_fused_args {
   float *partials;                   /* [256] per-CTA squared-norm partials */
   float *acc;                        /* [8] learn()-level statistic accumulators */
   int32_t *cur_idx;                  /* [B] */
-  unsigned int *barrier;             /* [64] grid-barrier counter + per-column-tile job counters (zeroed by the launcher) */
+  unsigned int *barrier;             /* [64] grid-barrier counter, per-row-tile P1 tickets, per-column-tile job counters (zeroed by the launcher) */
   long long *step;                   /* Adam step counter (device) */
   long long *cursor;                 /* minibatch cursor (device) */
   const float *lr;                   /* learning rate (device scalar) */

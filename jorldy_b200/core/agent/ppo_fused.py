@@ -15,7 +15,8 @@ class FusedArgs(ctypes.Structure):
         ("gW1", _P), ("gb1", _P), ("gW2", _P), ("gb2", _P), ("gWh", _P * 3), ("gbh", _P * 3),
         ("flat", _P), ("grad", _P), ("am", _P), ("av", _P), ("P4", ctypes.c_longlong),
         ("state", _P), ("action", _P), ("adv", _P), ("ret", _P), ("vold", _P), ("logp_old", _P), ("perm", _P),
-        ("h1", _P), ("h2", _P), ("xg", _P), ("w1p", _P), ("headp", _P), ("h2t", _P), ("W2t", _P), ("W2img", _P), ("W2Timg", _P), ("partials", _P), ("acc", _P),
+        ("h1", _P), ("h2", _P), ("xg", _P), ("w1p", _P), ("headp", _P),
+        ("dout", _P), ("dv2", _P), ("rowst", _P), ("h2t", _P), ("W2t", _P), ("W2img", _P), ("W2Timg", _P), ("partials", _P), ("acc", _P),
         ("cur_idx", _P), ("barrier", _P), ("step", _P), ("cursor", _P), ("lr", _P),
         ("peer", _P * 8), ("world", ctypes.c_int), ("rank", ctypes.c_int), ("xbase", ctypes.c_uint), ("xflag_off", ctypes.c_int), ("xgred_off", ctypes.c_int), ("xllin_off", ctypes.c_int),
         ("nh", ctypes.c_int * 3),
@@ -44,6 +45,7 @@ class FusedRunner:
         self.ws = {
             "h1": torch.empty(B, H, device=dev), "h2": torch.empty(B, H, device=dev), "xg": torch.empty(B, D, device=dev),
             "w1p": torch.zeros(B // 32, H, D + 1, device=dev), "headp": torch.zeros(H // 32, 2, B, 4, device=dev),
+            "dout": torch.zeros(B, 8, device=dev), "dv2": torch.zeros(B, device=dev), "rowst": torch.zeros(6, B, device=dev),
             "h2t": torch.empty(H // 32, B, 32, device=dev), "W2t": torch.empty(H // 32, H, 32, device=dev),
             "W2img": torch.empty(2, H // 32, H // 32, 1024, device=dev),
             "W2Timg": torch.empty(2, max(H // 128, 1), H // 32, 4096, device=dev),
@@ -76,6 +78,7 @@ class FusedRunner:
         a.adv, a.ret, a.vold, a.logp_old, a.perm = ptr(st["adv"]), ptr(st["ret"]), ptr(st["value"]), ptr(st["logp_old"]), ptr(st["perm"])
         ws = self.ws
         a.h1, a.h2, a.xg, a.w1p, a.headp = ptr(ws["h1"]), ptr(ws["h2"]), ptr(ws["xg"]), ptr(ws["w1p"]), ptr(ws["headp"])
+        a.dout, a.dv2, a.rowst = ptr(ws["dout"]), ptr(ws["dv2"]), ptr(ws["rowst"])
         a.h2t, a.W2t, a.W2img, a.W2Timg = ptr(ws["h2t"]), ptr(ws["W2t"]), ptr(ws["W2img"]), ptr(ws["W2Timg"])
         a.partials, a.acc, a.cur_idx, a.barrier = ptr(ws["partials"]), ptr(ag._acc), ptr(ws["cur_idx"]), ptr(ws["barrier"])
         a.step, a.cursor, a.lr = ptr(opt._step_dev), ptr(ag._cursor), ptr(opt._lr_dev)

@@ -5,7 +5,7 @@ are per-env-row and never cross ranks.  The reference has no counterpart (single
 actors only collect: manager/distributed_manager.py:7-65).
 
 `critic_loss = max(mean1, mean2)` (ppo.py:151-154): the in-kernel exchange makes the two means GLOBAL (the ranks swap
-their row sums during the row phase, csrc/ppo_fused.cu); only the NCCL fallback path (symmetric memory unavailable,
+their row sums right after the forward phase, csrc/ppo_fused.cu); only the NCCL fallback path (symmetric memory unavailable,
 JB_NO_P2P=1, CNN heads) still evaluates the max per rank on its local minibatch shard.
 """
 import torch

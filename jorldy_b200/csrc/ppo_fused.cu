@@ -11,11 +11,12 @@
 //       is GENERATED in shared memory from the gathered state rows (K = D <= 16), never read from HBM; the
 //       W2 panel arrives by cp.async.cg.  The epilogue also emits, per tile, the PARTIAL head outputs
 //       sum_{n in tile} h2[m, n] Wh[o, n], so that nobody has to re-read h2 rows to evaluate the heads.
-//   P3  row phase + backward.  Every CTA redundantly folds the partial head outputs of every minibatch
-//       row and runs the whole loss row math (ppo_rowmath.cuh, one thread per row): d loss/d head outputs
-//       of the minibatch end up in shared memory without a phase of their own (256 rows of ~300
-//       instructions cost less than a barrier).  Then the backward jobs, each with its panels prefetched
-//       while the previous job reduces:
+//       Every finished tile draws a ticket of its row tile; the CTA that draws the last one folds the row tile's
+//       partial head outputs and runs the loss row maths (ppo_rowmath.cuh, one thread per row) ONCE for those
+//       rows, into per-row tables in L2 (d loss/d head outputs, per-row statistics) that the barrier publishes.
+//   P3  critic means + backward.  Every CTA bulk-copies the d loss/d head outputs of the minibatch into shared
+//       memory and folds the per-row statistics into the two critic means.  Then the backward jobs, each with
+//       its panels prefetched while the previous job reduces (the first JB job's W2t panel before the barrier):
 //         JB  dh1 tile = ((dout Wh) * relu'(h2)) W2, masked by relu'(h1); dh2 is generated in place in the
 //             A panel; the epilogue turns the tile into PARTIAL dW1/db1 (x rows are <= 64 B each), so dh1
 //             never leaves the SM.
@@ -46,7 +47,7 @@
 //   Flag + fence protocols were slower: every hop paid a release store or system fence waiting for remote write
 //   acknowledgements plus acquire polls, and un-throttled relaxed polling of flags saturated L2.
 //   * the two scalar means of critic_loss = max(mean, mean) (ppo.py:151-154) are GLOBAL: each rank sends its two row sums to
-//     the peers during the row phase (two LL words); receiving step s's message from a peer also proves that the peer has
+//     the peers right after bar1 (two LL words); receiving step s's message from a peer also proves that the peer has
 //     finished step s-1.
 // No NCCL call between backward and Adam.
 //
@@ -72,6 +73,7 @@ constexpr int R2_FLOATS = JA_ROWS * 32;                 // 8192: a dense [256][3
 constexpr int MAX_B = 512;                              // minibatch rows (row-phase scratch in s_small)
 constexpr int ADAM_IT = 4;                              // float4 per thread kept in registers across the barrier
 constexpr int PS_FLOATS = (MAXO + 2) * PK;                // per-CTA parameter stash: head rows [MAXO][PK], b2, b1
+constexpr int CTR_ROW = 1;                              // a.barrier[CTR_ROW + mt]: finished P1 tiles of row tile mt (tickets)
 constexpr int CTR_JB = 32;                              // a.barrier[CTR_JB + kt]: finished JB jobs of column tile kt
 
 typedef jb_ppo_fused_args Args;
@@ -86,6 +88,10 @@ __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterp
 // the copy engine does the rest.)  Exactly one group of copies is in flight at a time: `Stager` tracks
 // the bytes of the group being issued and the phase parity of the barrier.
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
+// one 4-byte word global -> shared without a register: data fetched a whole tile ahead of its use
+__device__ __forceinline__ void cp_async4(float* dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
 struct Stager {
   unsigned mbar;      // shared-space address of the mbarrier
   unsigned bytes;     // bytes issued in the open group (uniform across the CTA)
@@ -379,7 +385,7 @@ template <bool TC, int NA, int ND>
 __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats, int flags /* debug: bit 8 = trace */) {
   extern __shared__ __align__(16) float smem[];
   float* s_small = smem;                       // SMALL_FLOATS
-  float* dsm = smem + SMALL_FLOATS;            // d loss/d head-outputs of the whole minibatch [B][MAXO]
+  float* dsm = smem + SMALL_FLOATS;            // d loss/d head-outputs of the whole minibatch [B][MAXO] (P1: rollout values)
   float* R0 = dsm + dsm_floats;                // RED_FLOATS: A panels of P1 / JB, split-K fold area, job scratch
   float* R1 = R0 + RED_FLOATS;                 // RED_FLOATS: B panels
   float* R2 = R1 + RED_FLOATS;                 // R2_FLOATS:  A panel of JA / JC; W1 during P1
@@ -481,12 +487,13 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
   for (long long i = lo + tid; i < hi; i += NT) shadow(i, p4[i]);   // published by the first grid barrier
   const float one_m_b1 = 1.f - a.beta1, one_m_b2 = 1.f - a.beta2;
 
-  auto issue_stage = [&](int job) {          // first-panel cp.async of a backward job (JD has none)
+  // first-panel cp.async of a backward job (JD has none); b_in_flight: a JB job's W2t panel was issued before bar1
+  auto issue_stage = [&](int job, bool b_in_flight) {
     if (job < nJB) {
       if (TC) return;                          // tensor-core dh1 jobs run their own operand rings
       const int mt = job / NTL, kt = job - mt * NTL;
       stage_kc(st, R0, a.h2, H, mt * 32, 0, H);
-      stage_block(st, R1, a.W2t + (size_t)kt * H * 32, H);
+      if (!b_in_flight) stage_block(st, R1, a.W2t + (size_t)kt * H * 32, H);
     } else if (job < nJB + nJA) {
       if (TC) return;                          // tensor-core dW2 jobs generate both operands
       const int j = job - nJB, nt = j / NP, kt0 = 2 * (j - nt * NP), kp = min(JA_ROWS, B);
@@ -501,24 +508,60 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
   // may the panels of `job` be fetched while the previous job still folds in R0?
   auto prefetchable = [&](int job) { return job < nJ3 && job >= nJB && (single || job >= nJB + nJA); };
 
-  // rollout rows of this thread's minibatch rows (row phase), one step ahead
-  int pr[2];
+  // ---- loss row maths, run for the rows of a P1 row tile by the CTA that finishes the tile's LAST column tile (it draws
+  // the last ticket of a.barrier[CTR_ROW + mt]; nobody waits on the tickets).  The rollout values of a row (adv, ret, v_old,
+  // log_prob_old, action: every row is visited once per epoch, so these are cold misses) are fetched at the start of the
+  // P1 tile by the thread that will need them, into dsm [6][RW] (dsm is free until bar1); the results go to global tables
+  // that bar1 publishes.
+  const int RW = TC ? 128 : 32;                        // rows of a P1 tile
+  auto gather_row = [&](int i, int r) {                // tile row i = rollout row r
+    cp_async4(dsm + i, a.adv + r); cp_async4(dsm + RW + i, a.ret + r); cp_async4(dsm + 2 * RW + i, a.vold + r);
+    if (!a.continuous) { cp_async4(dsm + 3 * RW + i, a.logp_old + r); cp_async4(dsm + 4 * RW + i, (const int32_t*)a.action + r); }
+    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    dsm[5 * RW + i] = __int_as_float(r);
+  };
+  auto row_maths = [&](int b, int i) {
+    const float g_adv = dsm[i], g_ret = dsm[RW + i], g_vold = dsm[2 * RW + i], g_lpo = dsm[3 * RW + i];
+    const int g_act = __float_as_int(dsm[4 * RW + i]), r = __float_as_int(dsm[5 * RW + i]);
+    float ov[2 * jbppo::MAX_A + 1];                     // row() indexes up to 2*MAX_A statically
 #pragma unroll
-  for (int q = 0; q < 2; ++q) pr[q] = tid + q * NT < B ? a.perm[cursor0 * (long long)B + tid + q * NT] : 0;
-  // ... and their rollout values (adv, ret, v_old, log_prob_old, action): gathered one phase ahead (every row is
-  // visited once per epoch, so these are cold misses), parked in dsm at the start of P1
-  float pg[2][5];
-  auto gather_rows = [&]() {
+    for (int o = 0; o < 2 * jbppo::MAX_A + 1; ++o) ov[o] = 0.f;
+#pragma unroll
+    for (int o = 0; o < MAXO; ++o) if (o < nout) ov[o] = hb[o];
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
-      if (tid + q * NT < B) {
-        const int r = pr[q];
-        pg[q][0] = a.adv[r]; pg[q][1] = a.ret[r]; pg[q][2] = a.vold[r];
-        if (!a.continuous) { pg[q][3] = a.logp_old[r]; pg[q][4] = __int_as_float(((const int32_t*)a.action)[r]); }
+      if (q < nq) {                                    // 16 independent loads in flight, folded in tile order
+        float4 v[PK / 32];
+#pragma unroll
+        for (int nt = 0; nt < PK / 32; ++nt)      // clamped, not predicated: all 16 loads go out back to back
+          v[nt] = ldcg4(a.headp + (((size_t)min(nt, NTL - 1) * 2 + q) * B + b) * 4);
+#pragma unroll
+        for (int nt = 0; nt < PK / 32; ++nt) {
+          if (nt < NTL) { ov[q * 4] += v[nt].x; ov[q * 4 + 1] += v[nt].y; ov[q * 4 + 2] += v[nt].z; ov[q * 4 + 3] += v[nt].w; }
+        }
       }
     }
+    jbppo::RowOut ro;
+    if (a.continuous)
+      jbppo::row<true, NA>(ov, A, 0, (const float*)a.action + (size_t)r * A, g_adv, g_ret, g_vold,
+                           a.logp_old + (size_t)r * A, hp, invB, ro);
+    else
+      jbppo::row<false, NA>(ov, A, g_act, nullptr, g_adv, g_ret, g_vold, &g_lpo, hp, invB, ro);
+    // d loss / d head outputs; the value head's slot holds the critic_loss1 candidate, resolved after bar1
+    float d[MAXO];
+#pragma unroll
+    for (int o = 0; o < MAXO; ++o) d[o] = o < npol ? ro.dpol[o] : (o == npol ? ro.dv1 : 0.f);
+    static_assert(MAXO == 8, "dout rows are two float4 ([B][8] in ppo_fused.py)");
+    float4* dst = reinterpret_cast<float4*>(a.dout + (size_t)b * MAXO);
+    dst[0] = make_float4(d[0], d[1], d[2], d[3]);
+    dst[1] = make_float4(d[4], d[5], d[6], d[7]);
+    a.dv2[b] = ro.dv2;
+    // the differences, not their squares: after bar1 the critic sums are `p += d * d`, one FMA per row (a stored square
+    // would be rounded once more)
+    float* st_ = a.rowst + b;
+    st_[0] = ro.d1; st_[B] = ro.d2; st_[2 * B] = ro.surr_min; st_[3 * B] = ro.ent; st_[4 * B] = ro.ratio; st_[5 * B] = ro.pmin;
   };
-  gather_rows();
+  int* tkt = reinterpret_cast<int*>(s_small + 1060);  // "this CTA drew the last ticket"
   // state rows of this CTA's first P1 tile of step 0 (later steps: gathered under the Adam phase)
   bool xs_ready = false;
   float xpre[ND];                                // TC: this thread's state row (row tid & 127 of the CTA's first tile)
@@ -559,15 +602,23 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     TR(28);
     stp.wait();
     TR(29);
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int b = tid + q * NT;
-      if (b < B) {
-        float* d = dsm + b * MAXO;
-        d[0] = pg[q][0]; d[1] = pg[q][1]; d[2] = pg[q][2]; d[5] = __int_as_float(pr[q]);
-        if (!a.continuous) { d[3] = pg[q][3]; d[4] = pg[q][4]; }
+    bool w2t_pre = false;                          // B panel of the first JB job already in flight (FFMA engine)
+    // one ticket per finished P1 tile of row tile mt: the CTA that draws the last one runs the row maths of the tile's rows
+    auto row_ticket = [&](int mt, bool mine, int b, int i) {
+      if (mine) asm volatile("cp.async.wait_all;\n" ::: "memory");   // the tile's rollout values (landed long ago)
+      __syncthreads();                             // every thread's headp stores happen-before thread 0's release
+      if (tid == 0) {
+        unsigned int old;
+        asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;\n" : "=r"(old) : "l"(a.barrier + CTR_ROW + mt) : "memory");
+        *tkt = old + 1u == (unsigned int)NTL * (unsigned int)(s + 1);
       }
-    }
+      __syncthreads();
+      TR(36);
+      if (*tkt) {
+        if (mine) row_maths(b, i);
+        TR(37);
+      }
+    };
     if constexpr (TC) {
       // ---- tensor-core forward: one 128 (minibatch rows) x 32 (hidden units) tile per job, K = H in chunks of 32.
       // A chunk = h1[128 rows][32 k] = relu(x W1^T + b1), GENERATED straight into the swizzled K-major layout (hi | lo of
@@ -603,6 +654,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           a.cur_idx[m0 + r] = xidx;
           for (int i = 0; i < D; ++i) a.xg[(size_t)(m0 + r) * D + i] = xr[i];
         }
+        if (half == 0) gather_row(r, xidx);
         // the tile's 128 input rows, transposed [ND][128], in the spare 8 KB behind the operand rings: the generator
         // below reads them as broadcast float4 (4 rows of one input feature)
         float* xt = tcp + ((TC_NA * TC_A_BYTES + TC_NB * TC_B_BYTES) >> 2);
@@ -713,6 +765,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // scratch reads above before later bulk copies / wgmma
         tc_g += (unsigned long long)NKC;
         TR(4);
+        row_ticket(mt, half == 0, m0 + r, r);
       }
     } else
     for (int job = cta; job < nJ1; job += (int)nctas) {
@@ -729,6 +782,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         for (int e = tid; e < 32 * MAXD; e += NT) { const int r = e >> 4, i = e & 15; xs[i * 32 + r] = i < D ? a.state[(size_t)sidx[r] * D + i] : 0.f; }
         __syncthreads();
       }
+      if (tid < 32) gather_row(tid, sidx[tid]);
       if (nt == 0) {
         if (tid < 32) a.cur_idx[m0 + tid] = sidx[tid];
         for (int e = tid; e < 32 * D; e += NT) { const int r = e / D, i = e - r * D; a.xg[(size_t)(m0 + r) * D + i] = xs[i * 32 + r]; }
@@ -787,6 +841,14 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       tile_mma<true, true>(R0, R1, H, acc, nullptr);
       __syncthreads();
       TR(3);
+      if (s > 0 && job + (int)nctas >= nJ1 && cta < nJB) {
+        // this CTA's last P1 product has released R1: the B panel of its first JB job goes out now; the job's h2 panel joins
+        // the same mbarrier group after bar1.  W2t is written by the Adam phase and published by bar5; step 0 has no bar5
+        // before it (the prologue's shadow writes are published by bar1), so step 0 issues the panel after bar1
+        const int kt = cta % NTL;
+        stage_block(st, R1, a.W2t + (size_t)kt * H * 32, H);
+        w2t_pre = true;
+      }
       float outv[4];
       tile_reduce<true, true>(acc, R0, outv);
       TR(4);
@@ -815,16 +877,22 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         const int r = lane >> 3, o = lane & 7;               // lane l holds value l = r * MAXO + o
         if (o < 4 * nq) a.headp[(((size_t)nt * 2 + (o >> 2)) * B + m0 + warp + 8 * r) * 4 + (o & 3)] = o < nout ? hv_[0] : 0.f;
       }
+      row_ticket(mt, tid < 32, m0 + tid, tid);
     }
     xs_ready = false;
     TR(5);
     grid_bar(a.barrier, epoch, nctas);
     TR(6);
 
-    // =========================== P3: row phase + backward jobs =========================================
+    // =========================== P3: critic means + backward jobs ======================================
+    // the per-row table that the row tiles' last arrivers wrote before bar1: one bulk copy per CTA (d loss / d head outputs
+    // into dsm, the second value-head candidate into dvs)
+    stp.bytes = (unsigned)B * (MAXO + 1) * 4u;
+    stp.commit();
+    if (tid == 0) { stp.copy(dsm, a.dout, (unsigned)B * MAXO * 4u); stp.copy(dvs, a.dv2, (unsigned)B * 4u); }
     int pre_job = -1;                              // job whose first panels are already in flight
-    if (cta < nJ3 && (cta < nJB || prefetchable(cta))) { issue_stage(cta); pre_job = cta; }
-    // tensor-core dh1 job: the first two W2^T chunks do not depend on the row phase, fetch them under it
+    if (cta < nJ3 && (cta < nJB || prefetchable(cta))) { issue_stage(cta, w2t_pre); pre_job = cta; }
+    // tensor-core dh1 job: the first two W2^T chunks do not depend on the row maths, fetch them under the critic sums
     auto jb_issue_a = [&](int kt4, int nc, unsigned long long g) {
       const unsigned slot = (unsigned)(g % TC_NA);
       const unsigned bar = tc_bar + 8u * (TC_BAR_JB + slot), dst = tc_base + slot * TC_A_BYTES;
@@ -833,7 +901,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       bulk_g2s(dst, src, 16384u, bar);
       bulk_g2s(dst + 16384u, src + (size_t)H * H, 16384u, bar);
     };
-    if (TC && cta >= nJB && cta < nJB + nJA) {     // dW2 job: all minibatch rows' inputs, transposed [D][B], under the row phase
+    if (TC && cta >= nJB && cta < nJB + nJA) {     // dW2 job: all minibatch rows' inputs, transposed [D][B]
       for (int e = tid; e < B * D; e += NT) { const int m = e / D, i = e - m * D; R2[i * B + m] = ldcg(a.xg + e); }
     }
     if (TC && cta < nJB && tid == 0) {
@@ -845,53 +913,19 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
     int next_r = 0;
     if (TC) { if (has_next) next_r = a.perm[(cursor0 + s + 1) * (long long)B + (cta / NTL) * 128 + (tid & 127)]; }
     else if (has_next && tid < 32) next_r = a.perm[(cursor0 + s + 1) * (long long)B + (cta / NTL) * 32 + tid];
-    if (s + 1 < a.n_steps) {
-#pragma unroll
-      for (int q = 0; q < 2; ++q) pr[q] = tid + q * NT < B ? a.perm[(cursor0 + s + 1) * (long long)B + tid + q * NT] : 0;
-    }
 
     float c1, c2;
     {
+      // the per-row statistics, folded exactly as one thread per row (rows tid, tid + NT) and then the warps in order
       float p1 = 0.f, p2 = 0.f, ssum = 0.f, esum = 0.f, mr = -INFINITY, mp = INFINITY;
 #pragma unroll 1
       for (int b = tid; b < B; b += NT) {
-        {
-          const float* d = dsm + b * MAXO;                    // parked in P1: adv, ret, v_old, log_prob_old, action, row id
-          const float g_adv = d[0], g_ret = d[1], g_vold = d[2], g_lpo = d[3];
-          const int g_act = __float_as_int(d[4]), r = __float_as_int(d[5]);
-          float ov[2 * jbppo::MAX_A + 1];                     // row() indexes up to 2*MAX_A statically
-#pragma unroll
-          for (int o = 0; o < 2 * jbppo::MAX_A + 1; ++o) ov[o] = 0.f;
-#pragma unroll
-          for (int o = 0; o < MAXO; ++o) if (o < nout) ov[o] = hb[o];
-#pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            if (q < nq) {                                    // 16 independent loads in flight, folded in tile order
-              float4 v[PK / 32];
-#pragma unroll
-              for (int nt = 0; nt < PK / 32; ++nt)      // clamped, not predicated: all 16 loads go out back to back
-                v[nt] = ldcg4(a.headp + (((size_t)min(nt, NTL - 1) * 2 + q) * B + b) * 4);
-#pragma unroll
-              for (int nt = 0; nt < PK / 32; ++nt) {
-                if (nt < NTL) { ov[q * 4] += v[nt].x; ov[q * 4 + 1] += v[nt].y; ov[q * 4 + 2] += v[nt].z; ov[q * 4 + 3] += v[nt].w; }
-              }
-            }
-          }
-          TR(31);
-          jbppo::RowOut ro;
-          if (a.continuous)
-            jbppo::row<true, NA>(ov, A, 0, (const float*)a.action + (size_t)r * A, g_adv, g_ret, g_vold,
-                             a.logp_old + (size_t)r * A, hp, invB, ro);
-          else
-            jbppo::row<false, NA>(ov, A, g_act, nullptr, g_adv, g_ret, g_vold, &g_lpo, hp, invB, ro);
-#pragma unroll
-          for (int o = 0; o < MAXO; ++o) dsm[b * MAXO + o] = o < npol ? ro.dpol[o] : 0.f;
-          dsm[b * MAXO + npol] = ro.dv1; dvs[b] = ro.dv2;      // the two candidate value-head gradients, resolved below
-          p1 += ro.sq1; p2 += ro.sq2; ssum += ro.surr_min; esum += ro.ent;
-          mr = fmaxf(mr, ro.ratio); mp = fminf(mp, ro.pmin);
-        }
+        const float d1 = ldcg(a.rowst + b), d2 = ldcg(a.rowst + B + b);
+        p1 = fmaf(d1, d1, p1); p2 = fmaf(d2, d2, p2);   // one FMA per row: the rounding of the sums is fixed, not left to
+                                                        // the compiler's mul/add contraction
+        ssum += ldcg(a.rowst + 2 * B + b); esum += ldcg(a.rowst + 3 * B + b);
+        mr = fmaxf(mr, ldcg(a.rowst + 4 * B + b)); mp = fminf(mp, ldcg(a.rowst + 5 * B + b));
       }
-      TR(32);
       p1 = jb_warp_sum(p1); p2 = jb_warp_sum(p2); ssum = jb_warp_sum(ssum); esum = jb_warp_sum(esum);
       mr = jb_warp_max(mr); mp = jb_warp_min(mp);
       if (lane == 0) { float* q = scr + warp * 8; q[0] = p1; q[1] = p2; q[2] = ssum; q[3] = esum; q[4] = mr; q[5] = mp; }
@@ -952,6 +986,8 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       c1 = t1 * invBW; c2 = t2 * invBW;
       float w1, w2;
       jbppo::critic_weights(c1, c2, w1, w2);
+      stp.wait();
+      TR(38);
       for (int b = tid; b < B; b += NT) dsm[b * MAXO + npol] = w1 * dsm[b * MAXO + npol] + w2 * dvs[b];
       if (cta == (int)nctas - 1 && tid == 0) {
         // learn()-level statistics of this minibatch (ppo.py:171-175), accumulated on the device
@@ -1017,7 +1053,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         __syncthreads();                                          // both warpgroups' products retired: tcs overlays A slot 1
         jbwg::store_acc_n32(acc, tcs, TC_LD);
         __syncthreads();
-        if (prefetchable(next)) { issue_stage(next); pre_job = next; }   // every MMA that read the rings has retired
+        if (prefetchable(next)) { issue_stage(next, false); pre_job = next; }   // every MMA that read the rings has retired
         {
           const int q = warp & 3, cb = (warp >> 2) * 16, kin = kin0 + q * 32 + lane;
           float rr[16];
@@ -1067,7 +1103,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         // ---- dh1 tile = ((dout Wh) * relu'(h2)) W2, masked by relu'(h1); partial dW1 / db1 ---------------
         const int mt = job / NTL, kt = job - mt * NTL;
         const int m0 = mt * 32, k0 = kt * 32;
-        if (pre_job != job) issue_stage(job);
+        if (pre_job != job) issue_stage(job, false);
         const int c4 = (tid & 127) * 4, rh = tid >> 7;
         float4 wr[MAXO];
 #pragma unroll
@@ -1095,7 +1131,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
         tile_mma<true, false>(R0, R1, H, acc, nullptr);
         __syncthreads();
         TR(14);
-        if (prefetchable(next)) { issue_stage(next); pre_job = next; }
+        if (prefetchable(next)) { issue_stage(next, false); pre_job = next; }
         float outv[4];
         tile_reduce<true, false>(acc, R0, outv);
         TR(15);
@@ -1261,7 +1297,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             const int kp = min(JA_ROWS, B - mp);
             if (!single || half == 0) {
               if (single) {
-                if (pre_job != job) issue_stage(job);
+                if (pre_job != job) issue_stage(job, false);
               } else {
                 __syncthreads();
                 stage_block(st, R2, a.h2t + ((size_t)nt * B + mp) * 32, kp);
@@ -1281,7 +1317,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           }
           __syncthreads();
           TR(19);
-          if (half == nhalf - 1 && prefetchable(next)) { issue_stage(next); pre_job = next; }
+          if (half == nhalf - 1 && prefetchable(next)) { issue_stage(next, false); pre_job = next; }
           float outv[4];
           tile_reduce<false, false>(acc, R0, outv);
           TR(20);
@@ -1330,7 +1366,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           }
         }
         __syncthreads();
-        if (prefetchable(next)) { issue_stage(next); pre_job = next; }
+        if (prefetchable(next)) { issue_stage(next, false); pre_job = next; }
         float* red = R0;               // [8][MAXO][32]
 #pragma unroll
         for (int o = 0; o < MAXO; ++o) red[(warp * MAXO + o) * 32 + lane] = hacc[o];
@@ -1488,7 +1524,6 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       }
       // ||g||: one coalesced read of the partials per CTA, then every warp folds them in the same fixed order
       if (a.world == 1 && tid < (int)nctas) dvs[tid] = ldcg(a.partials + tid);     // (multi-GPU: filled by the exchange above)
-      if (s + 1 < a.n_steps) gather_rows();        // next step's rollout values (row ids were loaded in P3)
       __syncthreads();
       float pv[NT / 32];
 #pragma unroll
@@ -1616,7 +1651,7 @@ JB_API int jb_ppo_fused_run(const void* host_args, void* stream) {
     for (int r = 0; r < a.world; ++r) if (!a.peer[r]) return JB_ERR_INVALID;
   }
   cudaStream_t s = (cudaStream_t)stream;
-  if (cudaMemsetAsync(a.barrier, 0, 64 * sizeof(unsigned int), s) != cudaSuccess) return JB_ERR_CUDA;   // grid counter + JB counters
+  if (cudaMemsetAsync(a.barrier, 0, 64 * sizeof(unsigned int), s) != cudaSuccess) return JB_ERR_CUDA;   // grid counter, row-tile tickets, JB counters: monotonic targets from 0
   const size_t smem = fused_smem(a.B);
   int dsm_floats = dsm_floats_for(a.B);
   int flags = 0;

@@ -24,6 +24,7 @@ struct RowOutW {
   float dpol[2 * W];       // d loss / d policy head outputs: discrete [A] logits; continuous [A] mu then [A] log_std
   float dv1, dv2;          // value-head gradient if critic_loss1 / critic_loss2 is the max (already x vf_coef / B)
   float sq1, sq2;          // (v - ret)^2, (v_clip - ret)^2
+  float d1, d2;            // v - ret, v_clip - ret
   float surr_min, ent;     // min(surr1, surr2), entropy (continuous: summed over dims)
   float ratio, pmin;       // ratio; exp(log_prob) (continuous: min over dims)
 };
@@ -79,6 +80,7 @@ __device__ __forceinline__ void row(const float* o, int A, int a_disc, const flo
   const float in_clip = (dv_raw >= -hp.eps_clip && dv_raw <= hp.eps_clip) ? 1.f : 0.f;
   const float d1 = v - ret, d2 = vclip - ret;
   r.sq1 = d1 * d1; r.sq2 = d2 * d2;
+  r.d1 = d1; r.d2 = d2;
   r.dv1 = hp.vf_coef * invB * 2.f * d1;
   r.dv2 = hp.vf_coef * invB * 2.f * d2 * in_clip;
 #pragma unroll

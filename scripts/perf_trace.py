@@ -39,11 +39,12 @@ print(f"{args.config} B={B}: {e0.elapsed_time(e1)/n*1000:.1f} us/step over {n} s
 tr = np.zeros((256, 48), np.int64)
 C.jb_ppo_fused_trace(tr.ctypes.data_as(ctypes.c_void_p))
 names = {0: "step start", 1: "P1 h1 generated", 2: "P1 panel landed", 3: "P1 mma", 4: "P1 reduce", 5: "P1 end", 6: "bar1",
-         7: "row phase done", 8: "P3 job0 start", 9: "P3 job1 start", 10: "P3 job2 start", 11: "P3 job3+ start",
+         7: "critic means done", 8: "P3 job0 start", 9: "P3 job1 start", 10: "P3 job2 start", 11: "P3 job3+ start",
          12: "JB staged", 13: "JB dh2 gen", 14: "JB mma", 15: "JB reduce", 16: "JB end",
          17: "JA staged", 18: "JA dh2 gen", 19: "JA mma(last)", 20: "JA reduce(last)", 21: "JA end",
-         22: "P3 jobs end", 28: "P1 stash issued", 29: "P1 stash landed", 31: "row: head outputs", 32: "row: math done",
-         33: "JB dW1 staged", 34: "JB dW1 stored", 35: "P1 shuffles done", 36: "row: perm issued", 23: "norm partial + p/m/v issued", 24: "bar3", 25: "P5 fold", 26: "P5 end", 27: "bar5"}
+         22: "P3 jobs end", 28: "P1 stash issued", 29: "P1 stash landed",
+         33: "JB dW1 staged", 34: "JB dW1 stored", 35: "P1 shuffles done", 36: "P1 ticket drawn",
+         37: "row maths done (last arriver)", 38: "row table landed", 23: "norm partial + p/m/v issued", 24: "bar3", 25: "P5 fold", 26: "P5 end", 27: "bar5"}
 ghz = args.ghz
 n = int((tr[:, 0] > 0).sum())               # CTAs of the launch
 for cta in sorted({0, n // 2, n - 1}):

@@ -29,7 +29,7 @@ for rep in range(3):
         print(f"world {world}: {e0.elapsed_time(e1)/n*1000:.1f} us/step over {n} steps", flush=True)
 tr = np.zeros((256, 48), np.int64)
 C.jb_ppo_fused_trace(tr.ctypes.data_as(ctypes.c_void_p))
-names = {0: "step start", 5: "P1 end", 6: "bar1", 31: "row: head outputs", 32: "row: math done", 40: "row: critic sums of all ranks", 7: "row phase done",
+names = {0: "step start", 5: "P1 end", 6: "bar1", 36: "P1 ticket drawn", 37: "row maths done (last arriver)", 38: "row table landed", 40: "critic sums of all ranks", 7: "critic means done",
          16: "JB end", 21: "JA end", 22: "P3 jobs end", 23: "p/m/v issued", 24: "bar3", 41: "X: peers' gradients complete (F1)",
          42: "X: chunk averaged + stored to all ranks", 43: "X: chunk tag published", 44: "X: all chunks of all owners landed",
          25: "P5 fold", 26: "P5 end", 27: "bar5"}
