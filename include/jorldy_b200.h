@@ -325,6 +325,27 @@ JB_API int jb_iqn_mul_bwd(const float* dz, const float* psi, const float* phi, i
                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Rainbow-IQN (Toromanoff et al. arXiv:1908.04683: IQN with Rainbow's double-Q, n-step targets and prioritised replay),
+ * csrc/quantile.cu.  [B, N, A] layout only: pred [B, N, A] (online on s), next_online [B, Nn, A] (online on s'),
+ * next_target [B, Np, A] (target on s'), tau [B, N], reward / done [B, n_step].
+ *   a*   = argmax_a mean_j next_online[b, j, a], first index on ties (double-Q);
+ *   y_j  = fold_{s = n_step-1 .. 0} (r_s + ((1 - d_s) gamma) y), from y = next_target[b, j, a*]  (c51.cu's float order);
+ *   L_b  = (1/Np) sum_j sum_i |tau_i - 1{u_ij < 0}| smooth_l1(u_ij), u_ij = y_j - pred[b, i, a_b]   (kappa = 1);
+ *   dpred[b, i, a_b] = -(w_b / (B Np)) sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -1, 1), 0 on every other action;
+ *   loss [B] = the unweighted L_b, prio [B] (f64, may be NULL) = L_b^alpha, a_star [B] (may be NULL);
+ *   stats = {(1/B) sum_b w_b L_b, max_{b,a} mean_i pred, max pred, min pred}; scratch: 4*B floats.
+ * weights [B] are the f64 IS weights, each sample its own (NULL = all ones).  1 <= A <= 18, 1 <= N, Nn, Np <= 256,
+ * n_step >= 1, else JB_ERR_INVALID.  One CTA per sample, fixed-order sums, a single-thread finalize: bit-reproducible.
+ * With n_step = 1, next_online == next_target and weights NULL (or all ones), dpred, loss, a_star and stats[0..1] equal
+ * jb_quantile_loss's on the [B, N, A] layout bit for bit.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_rainbow_iqn_loss(const float* pred, const float* next_online, const float* next_target, const float* tau,
+                               const void* action, int action_kind, const float* reward, const float* done,
+                               const double* weights, int B, int A, int N, int Nn, int Np, int n_step, float gamma,
+                               float alpha, float* dpred, float* loss, double* prio, int32_t* a_star, float* stats,
+                               float* scratch, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Munchausen RL (M-DQN, M-IQN; Vieillard, Pietquin, Geist 2020, arXiv:2007.14430), csrc/munchausen.cuh with
  * csrc/dqn.cu and csrc/quantile.cu.  q'(s, .) and q'(s', .) are the TARGET network's Q; tau is the entropy temperature
  * (m_tau), alpha the Munchausen scale (m_alpha), l0 the clip floor.  Per sample, one thread, actions ascending:

@@ -3,7 +3,7 @@
 `load("config.<agent>.<env>")` returns a module-like namespace with the four dicts the reference's
 config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / train).  Values follow the
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
-per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
+per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
@@ -38,7 +38,13 @@ _VALUE_AGENTS = {
     "m_dqn": ("discrete_q_network", dict(_EPS, alpha=0.9, tau=0.03, l_0=-1), 10, 32),
     "m_iqn": ("iqn", dict(_EPS, num_sample=64, embedding_dim=64, sample_min=0.0, sample_max=1.0, alpha=0.9, tau=0.03, l_0=-1),
               10, 32),
+    # Rainbow-IQN (arXiv:1908.04683): Rainbow's row without the support, plus IQN's fraction counts; not compared with the
+    # reference's config/rainbow_iqn/*.py, which takes precedence when a JORLDY config directory is on sys.path
+    "rainbow_iqn": ("rainbow_iqn", dict(n_step=3, alpha=0.5, beta=0.4, learn_period=2, uniform_sample_prob=1e-3,
+                                        noise_type="factorized", num_sample=64, embedding_dim=64, sample_min=0.0,
+                                        sample_max=1.0), 10, 8),
 }
+_RAINBOW_ATARI = ("rainbow", "rainbow_iqn")      # learn_period 4, lr 2.5e-4 / 4 and 30 M steps on Atari
 
 
 def _value_config(agent, env):
@@ -48,11 +54,11 @@ def _value_config(agent, env):
         a.update(extra)
         if "epsilon_min" in a:
             a.update(epsilon_min=0.1, explore_ratio=0.1)
-        if agent == "rainbow":
+        if agent in _RAINBOW_ATARI:
             a.update(learn_period=4)
-        lr = 2.5e-4 / 4 if agent == "rainbow" else 1e-4
+        lr = 2.5e-4 / 4 if agent in _RAINBOW_ATARI else 1e-4
         return dict(env=dict(_ATARI_ENV), agent=a, optim=dict(name="adam", lr=lr),
-                    train=dict(_TRAIN_ATARI, run_step=30000000 if agent == "rainbow" else 10000000,
+                    train=dict(_TRAIN_ATARI, run_step=30000000 if agent in _RAINBOW_ATARI else 10000000,
                                update_period=32, num_workers=16))
     a = dict(name=agent, network=net, **_REPLAY)
     a.update(extra)

@@ -6,10 +6,11 @@ from .dqn import DQN, Double, Dueling, Multistep, PER, Noisy, C51, Rainbow, ApeX
 from .ddpg import DDPG, TD3, SAC
 from .quantile import IQN, QRDQN
 from .munchausen import MDQN, MIQN
+from .rainbow_iqn import RainbowIQN
 
 agent_dict = OrderedDict(sorted(dict(ape_x=ApeX, c51=C51, ddpg=DDPG, double=Double, dqn=DQN, dueling=Dueling, iqn=IQN,
                                      m_dqn=MDQN, m_iqn=MIQN, multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, qrdqn=QRDQN,
-                                     rainbow=Rainbow, sac=SAC, td3=TD3).items()))
+                                     rainbow=Rainbow, rainbow_iqn=RainbowIQN, sac=SAC, td3=TD3).items()))
 
 
 def register(name, cls):

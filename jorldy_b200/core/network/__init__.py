@@ -8,6 +8,7 @@ from .iqn import IQN
 from .noisy import Noisy, Rainbow
 from .policy import ContinuousPolicy, DeterministicPolicy, DiscretePolicy
 from .q_network import ContinuousQ_Network
+from .rainbow_iqn import RainbowIQN
 
 network_dict = OrderedDict(
     continuous_policy=ContinuousPolicy,
@@ -21,6 +22,7 @@ network_dict = OrderedDict(
     iqn=IQN,
     noisy=Noisy,
     rainbow=Rainbow,
+    rainbow_iqn=RainbowIQN,
 )
 
 

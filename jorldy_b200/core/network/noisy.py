@@ -39,8 +39,8 @@ class _NoisyMixin:
         self.noise_seed = int(seed) if seed is not None else 0
         self._draw_ctr = torch.zeros(1, dtype=torch.int64, device=self.device)
 
-    def _noisy_fwd(self, x, tag, lt, layer_id, in_f, out_f, y, relu, is_train, noise):
-        """y = act(x @ (mu + sig*eps_w) + (mu_b + sig_b*eps_b)); keeps W/f vectors under `tag+lt`."""
+    def _noisy_make(self, tag, lt, layer_id, in_f, out_f, is_train, noise):
+        """Draws one layer's factors (or takes injected normals) and returns its effective (W, b), kept under `tag+lt`."""
         p = self.p
         fi = self._buf(tag + lt + ".fi", (in_f,)); fj = self._buf(tag + lt + ".fj", (out_f,))
         w = self._buf(tag + lt + ".w", (in_f, out_f)); b = self._buf(tag + lt + ".b", (out_f,))
@@ -48,6 +48,11 @@ class _NoisyMixin:
         C.jb_noisy_make(ptr(p[f"mu_w{lt}"]), ptr(p[f"sig_w{lt}"]), ptr(p[f"mu_b{lt}"]), ptr(p[f"sig_b{lt}"]), in_f, out_f,
                         ptr(ei), ptr(ej), self.noise_seed, layer_id, ptr(self._draw_ctr), int(is_train), ptr(fi), ptr(fj),
                         ptr(w), ptr(b), stream_ptr())
+        return w, b
+
+    def _noisy_fwd(self, x, tag, lt, layer_id, in_f, out_f, y, relu, is_train, noise):
+        """y = act(x @ (mu + sig*eps_w) + (mu_b + sig_b*eps_b)); keeps W/f vectors under `tag+lt`."""
+        w, b = self._noisy_make(tag, lt, layer_id, in_f, out_f, is_train, noise)
         L.linear_io_fwd(x, w, b, y, relu=relu)
 
     def _noisy_bwd(self, dy, x, tag, lt, in_f, out_f, dx, relu_act):

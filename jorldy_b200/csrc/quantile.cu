@@ -9,7 +9,8 @@
 //   d loss / d theta_i = -(1/(B N')) sum_j |tau_i - 1{u_ij < 0}| clamp(u_ij, -1, 1)  (0 on non-taken actions)
 // a* = argmax_a mean_j theta'_j(s', a), first index on ties.  Every sum runs in a fixed order (no atomics), and the
 // batch statistics are folded by one thread, so a learn() is bit-reproducible.  M-IQN's loss (arXiv:2007.14430) runs the
-// same per-sample Huber loop on Munchausen targets (munchausen.cuh).
+// same per-sample Huber loop on Munchausen targets (munchausen.cuh), and Rainbow-IQN's (arXiv:1908.04683) on double-Q
+// n-step targets with per-sample importance weights and new priorities.
 #include "common.cuh"
 #include "munchausen.cuh"
 #include "philox.cuh"
@@ -148,6 +149,75 @@ munchausen_quantile_loss_kernel(const float* __restrict__ pred, const float* __r
   }
 }
 
+// Rainbow-IQN (arXiv:1908.04683) on the [B, N, A] layout: a* = argmax_a mean_j next_online[b, j, a] (double-Q, first index
+// on ties), the n-step target y_j = fold_{s = n-1 .. 0} (r_s + ((1 - d_s) gamma) y) from y = next_target[b, j, a*] in c51.cu's
+// float order, and quantile_huber, unchanged, with the sample's own IS weight in gcoef = w_b / (B Np).  loss_out holds the
+// unweighted L_b, prio L_b^alpha; partial[b] = {w_b L_b, max_a mean_i pred, max pred, min pred}.
+__global__ void __launch_bounds__(QT)
+rainbow_iqn_loss_kernel(const float* __restrict__ pred, const float* __restrict__ next_online,
+                        const float* __restrict__ next_target, const float* __restrict__ tau, const void* __restrict__ action,
+                        int action_kind, const float* __restrict__ reward, const float* __restrict__ done,
+                        const double* __restrict__ weights, int B, int A, int N, int Nn, int Np, int n_step, float gamma,
+                        float alpha, float* __restrict__ dpred, float* __restrict__ loss_out, double* __restrict__ prio,
+                        int32_t* __restrict__ a_star_out, float* __restrict__ partial /*[B][4]*/) {
+  __shared__ float s_y[QMAXN], s_tau[QMAXN], s_qn[QMAXA], s_qo[QMAXA], s_red[QT / 32], s_mx[QT / 32], s_mn[QT / 32];
+  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* pb = pred + (size_t)b * A * N;
+  const float* ob = next_online + (size_t)b * A * Nn;
+  const float* tb = next_target + (size_t)b * A * Np;
+  // rows 0 .. A-1: the online means on s (max_Q); rows A .. 2A-1: the online means on s' (a*)
+  for (int e = warp; e < 2 * A; e += QT / 32) {
+    const int k = e / A, a = e - k * A;
+    const float v = k == 0 ? warp_mean(pb + a, A, N, lane) : warp_mean(ob + a, A, Nn, lane);
+    if (lane == 0) (k == 0 ? s_qo : s_qn)[a] = v;
+  }
+  float mx = -INFINITY, mn = INFINITY;
+  for (int e = tid; e < A * N; e += QT) { const float v = pb[e]; mx = fmaxf(mx, v); mn = fminf(mn, v); }
+  mx = jb_warp_max(mx);
+  mn = jb_warp_min(mn);
+  if (lane == 0) { s_mx[warp] = mx; s_mn[warp] = mn; }
+  for (int i = tid; i < N; i += QT) s_tau[i] = tau[(size_t)b * N + i];
+  __syncthreads();
+  int a_star = 0;
+  float best = s_qn[0];
+  for (int a = 1; a < A; ++a)
+    if (s_qn[a] > best) { best = s_qn[a]; a_star = a; }
+  const float* rr = reward + (size_t)b * n_step;
+  const float* dr = done + (size_t)b * n_step;
+  for (int j = tid; j < Np; j += QT) {
+    float y = tb[(size_t)j * A + a_star];
+    for (int s = n_step - 1; s >= 0; --s) y = __fadd_rn(rr[s], __fmul_rn(__fmul_rn(__fadd_rn(1.f, -dr[s]), gamma), y));
+    s_y[j] = y;
+  }
+  const int a_t = read_action(action, action_kind, b);
+  const double w = weights ? weights[b] : 1.0;
+  const float gcoef = (float)(w / ((double)B * (double)Np));
+  __syncthreads();
+  const float lb = quantile_huber(pb, 1, A, s_y, s_tau, s_red, A, N, Np, a_t, gcoef, dpred + (size_t)b * A * N);
+  if (tid == 0) {
+    float maxq = s_qo[0];
+    for (int a = 1; a < A; ++a) maxq = fmaxf(maxq, s_qo[a]);
+    for (int k = 1; k < QT / 32; ++k) { mx = fmaxf(mx, s_mx[k]); mn = fminf(mn, s_mn[k]); }
+    loss_out[b] = lb;
+    if (prio) prio[b] = pow((double)lb, (double)alpha);
+    if (a_star_out) a_star_out[b] = a_star;
+    partial[4 * b] = (float)(w * (double)lb);
+    partial[4 * b + 1] = maxq;
+    partial[4 * b + 2] = mx;
+    partial[4 * b + 3] = mn;
+  }
+}
+
+__global__ void rainbow_iqn_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
+  if (threadIdx.x != 0) return;
+  float l = 0.f, mq = -INFINITY, ml = -INFINITY, nl = INFINITY;
+  for (int b = 0; b < B; ++b) {
+    l += partial[4 * b];
+    mq = fmaxf(mq, partial[4 * b + 1]); ml = fmaxf(ml, partial[4 * b + 2]); nl = fminf(nl, partial[4 * b + 3]);
+  }
+  stats[0] = l / (float)B; stats[1] = mq; stats[2] = ml; stats[3] = nl;
+}
+
 __global__ void quantile_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
   if (threadIdx.x != 0) return;
   float l = 0.f, mq = -INFINITY;
@@ -200,6 +270,23 @@ JB_API int jb_munchausen_quantile_loss(const float* pred, const float* next_targ
                                                    reward, done, A, N, Np, Nc, gamma, m_alpha, m_tau, l0, gcoef, dpred,
                                                    scratch);
   quantile_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  return jb_check_launch();
+}
+
+JB_API int jb_rainbow_iqn_loss(const float* pred, const float* next_online, const float* next_target, const float* tau,
+                               const void* action, int action_kind, const float* reward, const float* done,
+                               const double* weights, int B, int A, int N, int Nn, int Np, int n_step, float gamma,
+                               float alpha, float* dpred, float* loss, double* prio, int32_t* a_star, float* stats,
+                               float* scratch, void* stream) {
+  if (!pred || !next_online || !next_target || !tau || !action || !reward || !done || !dpred || !loss || !stats || !scratch)
+    return JB_ERR_INVALID;
+  if (B <= 0 || A <= 0 || A > QMAXA || N <= 0 || N > QMAXN || Nn <= 0 || Nn > QMAXN || Np <= 0 || Np > QMAXN ||
+      n_step < 1 || action_kind < 0 || action_kind > 2)
+    return JB_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  rainbow_iqn_loss_kernel<<<B, QT, 0, s>>>(pred, next_online, next_target, tau, action, action_kind, reward, done, weights, B,
+                                           A, N, Nn, Np, n_step, gamma, alpha, dpred, loss, prio, a_star, scratch);
+  rainbow_iqn_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }
 
