@@ -213,7 +213,8 @@ JB_API int jb_c51_loss(const float* logits, const float* next_online, const floa
 JB_API int jb_c51_q(const float* logits, const float* z, int M, int A, int K, float* q, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * NoisyNet — jorldy/core/network/utils.py:55-86 (noisy_l), factorised noise.
+ * NoisyNet — jorldy/core/network/utils.py:55-86 (noisy_l), factorised noise.  A drawn (not injected) layer
+ * needs in_f + out_f <= 8192, else JB_ERR_INVALID: Philox counter = draw * 4096 + factor / 2.
  * ------------------------------------------------------------------------------------------- */
 JB_API int jb_noisy_make(const float* mu_w, const float* sig_w, const float* mu_b, const float* sig_b, int in_f,
                          int out_f, const float* eps_i, const float* eps_j, uint64_t seed, uint64_t stream_id,

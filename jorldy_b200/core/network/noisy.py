@@ -4,7 +4,8 @@
 Noisy tensors keep the reference layout (in, out) and parameter order (the direct nn.Parameters
 precede the sub-modules in state_dict(), SURVEY.md Appendix B).  Every forward draws fresh factor
 noise (utils.py:59-68) through jb_noisy_make — Philox stream = layer index, device-side draw
-counter — or takes injected normals `noise=[(eps_i, eps_j), ...]` for parity tests.
+counter — or takes injected normals `noise=[(eps_i, eps_j), ...]` for parity tests.  forward_rows
+(act()) draws once per call and runs every chunk of rows on those weights.
 """
 import torch
 
@@ -50,11 +51,6 @@ class _NoisyMixin:
                         ptr(w), ptr(b), stream_ptr())
         return w, b
 
-    def _noisy_fwd(self, x, tag, lt, layer_id, in_f, out_f, y, relu, is_train, noise):
-        """y = act(x @ (mu + sig*eps_w) + (mu_b + sig_b*eps_b)); keeps W/f vectors under `tag+lt`."""
-        w, b = self._noisy_make(tag, lt, layer_id, in_f, out_f, is_train, noise)
-        L.linear_io_fwd(x, w, b, y, relu=relu)
-
     def _noisy_bwd(self, dy, x, tag, lt, in_f, out_f, dx, relu_act):
         """Gradients of one noisy layer: fills g[mu/sig], returns dx (masked by relu_act>0) if dx given."""
         g = self.g
@@ -85,23 +81,33 @@ class Noisy(FlatNetwork, _NoisyMixin):
             _noisy_init(self.p, "1", F, D_hidden, noise_type, gen)
             _noisy_init(self.p, "2", D_hidden, D_out, noise_type, gen)
 
-    def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
-        M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
+    def _make_noise(self, tag, is_train, noise):
+        """Effective (W, b) of the two noisy layers in call order; noise: injected [(eps_i, eps_j)] x 2."""
         F, H, A = self.head.D_head_out, self.D_hidden, self.D_out
         n1, n2 = noise if noise is not None else (None, None)
+        return {"1": self._noisy_make(tag, "1", 1, F, H, is_train, n1), "2": self._noisy_make(tag, "2", 2, H, A, is_train, n2)}
+
+    def _body(self, x, idx, M, wb, tag, out, save):
         feat = self.head.forward(self, x, idx, M, tag, save)
-        h = self._buf(tag + "h", (M, H))
-        self._noisy_fwd(feat, tag, "1", 1, F, H, h, True, is_train, n1)
+        h = self._buf(tag + "h", (M, self.D_hidden))
+        L.linear_io_fwd(feat, *wb["1"], h, relu=True)
         if out is None:
-            out = self._buf(tag + "q", (M, A))
-        self._noisy_fwd(h, tag, "2", 2, H, A, out, False, is_train, n2)
+            out = self._buf(tag + "q", (M, self.D_out))
+        L.linear_io_fwd(h, *wb["2"], out, relu=False)
         return out
 
+    def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
+        M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
+        return self._body(x, idx, M, self._make_noise(tag, is_train, noise), tag, out, save)
+
     def forward_rows(self, x, out, is_train=True, noise=None):
+        """Chunked inference (act() over many env rows): one noise draw for the whole call, every chunk on the same
+        effective weights, as the reference's act() draws once per call."""
         M = x.shape[0]
+        wb = self._make_noise("inf.", is_train, noise)
         for s in range(0, M, self.head.max_rows):
             e = min(M, s + self.head.max_rows)
-            self.forward(x[s:e], is_train, None, e - s, out[s:e], tag=f"inf{e - s}.", save=False, noise=noise)
+            self._body(x[s:e], None, e - s, wb, f"inf{e - s}.", out[s:e], False)
         return out
 
     def backward(self, dq, M, tag="t."):
@@ -136,31 +142,43 @@ class Rainbow(FlatNetwork, _NoisyMixin):
             _noisy_init(self.p, "_a2", H, N_atom * D_out, noise_type, gen)
             _noisy_init(self.p, "_v2", H, N_atom, noise_type, gen)
 
-    def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
-        """Returns logits [M, A, K].  noise order = the reference's call order: a1, v1, a2, v2."""
-        M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
+    def _make_noise(self, tag, is_train, noise):
+        """Effective (W, b) of the four noisy layers in the reference's call order a1, v1, a2, v2 (Philox streams 1..4);
+        noise: injected [(eps_i, eps_j)] x 4."""
+        H, AK, K = self.D_hidden, self.D_out * self.N_atom, self.N_atom
+        dims = (("_a1", 1, H, H), ("_v1", 2, H, H), ("_a2", 3, H, AK), ("_v2", 4, H, K))
+        noise = noise if noise is not None else (None,) * 4
+        return {lt: self._noisy_make(tag, lt, lid, i, o, is_train, nz) for (lt, lid, i, o), nz in zip(dims, noise)}
+
+    def _body(self, x, idx, M, wb, tag, out, save):
         H, A, K = self.D_hidden, self.D_out, self.N_atom
-        na1, nv1, na2, nv2 = noise if noise is not None else (None,) * 4
         feat = self.head.forward(self, x, idx, M, tag, save)
         f = self._buf(tag + "f", (M, H))
         L.linear_fwd(feat, self.p["l.weight"], self.p["l.bias"], f, relu=True)
         xa = self._buf(tag + "xa", (M, H)); xv = self._buf(tag + "xv", (M, H))
-        self._noisy_fwd(f, tag, "_a1", 1, H, H, xa, True, is_train, na1)
-        self._noisy_fwd(f, tag, "_v1", 2, H, H, xv, True, is_train, nv1)
+        L.linear_io_fwd(f, *wb["_a1"], xa, relu=True)
+        L.linear_io_fwd(f, *wb["_v1"], xv, relu=True)
         a = self._buf(tag + "a", (M, A * K)); v = self._buf(tag + "v", (M, K))
-        self._noisy_fwd(xa, tag, "_a2", 3, H, A * K, a, False, is_train, na2)
-        self._noisy_fwd(xv, tag, "_v2", 4, H, K, v, False, is_train, nv2)
+        L.linear_io_fwd(xa, *wb["_a2"], a, relu=False)
+        L.linear_io_fwd(xv, *wb["_v2"], v, relu=False)
         if out is None:
             out = self._buf(tag + "logits", (M, A, K))
         C.jb_dueling_fwd(ptr(a), ptr(v), M, A, K, ptr(out), stream_ptr())
         return out
 
+    def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
+        """Returns logits [M, A, K].  noise order = the reference's call order: a1, v1, a2, v2."""
+        M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
+        return self._body(x, idx, M, self._make_noise(tag, is_train, noise), tag, out, save)
+
     def forward_rows(self, x, out, is_train=True, noise=None):
-        """Chunked inference (act() over many env rows); out [M, A, K].  noise: injected draws (parity tests)."""
+        """Chunked inference (act() over many env rows); out [M, A, K].  One noise draw for the whole call, every chunk
+        on the same effective weights (the reference's act() draws once per call).  noise: injected draws (parity tests)."""
         M = x.shape[0]
+        wb = self._make_noise("inf.", is_train, noise)
         for s in range(0, M, self.head.max_rows):
             e = min(M, s + self.head.max_rows)
-            self.forward(x[s:e], is_train, None, e - s, out[s:e], tag=f"inf{e - s}.", save=False, noise=noise)
+            self._body(x[s:e], None, e - s, wb, f"inf{e - s}.", out[s:e], False)
         return out
 
     def backward(self, dlogits, M, tag="t."):

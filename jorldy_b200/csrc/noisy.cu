@@ -14,6 +14,13 @@
 
 namespace {
 
+// Philox counter of a drawn factor t (t < in_f: f_i[t], else f_j[t - in_f]) = draw * DRAW_STRIDE + t / 2: one Philox
+// block gives two normals, so one draw owns 2 * DRAW_STRIDE normals.  A layer with in_f + out_f > 2 * DRAW_STRIDE would
+// run into the next draw's counters and successive draws would share normals, so jb_noisy_make rejects it when it
+// draws (injected normals have no such limit).  Widening the stride would change every existing stream.
+constexpr uint64_t DRAW_STRIDE = 4096;
+constexpr int MAX_DRAWN_FACTORS = 2 * (int)DRAW_STRIDE;
+
 __device__ __forceinline__ float f_noise(float e) { return (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f)) * sqrtf(fabsf(e)); }
 
 // f_i[in], f_j[out] from injected normals or Philox Box-Muller (stream = layer id, ctr = draw index)
@@ -28,7 +35,7 @@ __global__ void noisy_factors_kernel(const float* __restrict__ eps_i, const floa
   if (inj) e = (t < in_f) ? eps_i[t] : eps_j[t - in_f];
   else {
     const uint64_t c = ctr_ptr ? (uint64_t)(*ctr_ptr) : 0;
-    jb_philox4 r = jb_philox(seed, stream, c * 4096 + (uint64_t)(t >> 1));
+    jb_philox4 r = jb_philox(seed, stream, c * DRAW_STRIDE + (uint64_t)(t >> 1));
     const float u1 = (float)((r.x >> 8) + 1u) * (1.0f / 16777216.0f), u2 = jb_u01_float(r.y);
     const float rad = sqrtf(-2.0f * logf(u1));
     e = (t & 1) ? rad * sinpif(2.0f * u2) : rad * cospif(2.0f * u2);
@@ -72,16 +79,19 @@ __global__ void noisy_grad_kernel(const float* __restrict__ dw_eff, const float*
 
 // Draws the factor vectors (eps_i/eps_j injected normals, or Philox with stream id + device draw
 // counter) and materialises W [in,out], b [out].  is_train = 0 -> W = mu_w, b = mu_b (utils.py:69-71).
+// Drawing (either eps pointer NULL) needs in_f + out_f <= 8192 (see DRAW_STRIDE) and bumps *draw_ctr once.
 JB_API int jb_noisy_make(const float* mu_w, const float* sig_w, const float* mu_b, const float* sig_b, int in_f,
                          int out_f, const float* eps_i, const float* eps_j, uint64_t seed, uint64_t stream_id,
                          long long* draw_ctr, int is_train, float* f_i, float* f_j, float* w_eff, float* b_eff,
                          void* stream) {
   if (!mu_w || !sig_w || !mu_b || !sig_b || !f_i || !f_j || !w_eff || !b_eff || in_f <= 0 || out_f <= 0)
     return JB_ERR_INVALID;
+  const bool draws = is_train && !(eps_i && eps_j);
+  if (draws && (long long)in_f + out_f > MAX_DRAWN_FACTORS) return JB_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   if (is_train) {
     noisy_factors_kernel<<<jb_div_up(in_f + out_f, 128), 128, 0, s>>>(eps_i, eps_j, in_f, out_f, seed, stream_id, draw_ctr, f_i, f_j);
-    if (draw_ctr && !(eps_i && eps_j)) noisy_bump_kernel<<<1, 32, 0, s>>>(draw_ctr);
+    if (draw_ctr && draws) noisy_bump_kernel<<<1, 32, 0, s>>>(draw_ctr);
   } else {
     cudaMemsetAsync(f_i, 0, sizeof(float) * in_f, s);
     cudaMemsetAsync(f_j, 0, sizeof(float) * out_f, s);
