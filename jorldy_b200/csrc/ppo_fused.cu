@@ -316,6 +316,20 @@ __device__ __forceinline__ float block_sum(float v, float* scratch /*[8]*/) {
   return t;
 }
 
+// one level of the head-output butterfly: lanes with bit N set keep the upper half of values [0, 2N), the others the
+// lower half, and each adds the half its partner sent.  One template instance per level so that every index into h is a
+// compile-time constant: a loop over the levels left h in local memory (a load-shuffle-store round trip per value).
+__device__ __forceinline__ float butterfly_pair(float lo, float hi, bool up, int N) {
+  return (up ? hi : lo) + __shfl_xor_sync(0xffffffffu, up ? lo : hi, N);
+}
+template <int N, int S>
+__device__ __forceinline__ void butterfly_level(float (&h)[S], int lane) {
+  static_assert(2 * N <= S, "butterfly level wider than its values");
+  const bool up = (lane & N) != 0;
+#pragma unroll
+  for (int q = 0; q < N; ++q) h[q] = butterfly_pair(h[q], h[q + N], up, N);
+}
+
 // d (loss) / d (h2 pre-activation) for 4 adjacent columns of one row: (dout[row] . Wh[:, c..c+3]) * relu'(h2)
 __device__ __forceinline__ float4 dh2_quad(const float* drow, const float4 (&wr)[MAXO], float4 hv) {
   const float4 d0 = *reinterpret_cast<const float4*>(drow);
@@ -855,24 +869,23 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
       {
         // 32 per-lane values (4 rows x MAXO products) -> lane l ends with the warp total of value l: a butterfly
         // that halves the value count at every step (31 shuffles, fixed order) instead of 5 shuffles per value
-        float hv_[32];
+        float v[4];
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-          const float v = fmaxf(outv[r] + b2v, 0.f);
-          a.h2[(size_t)(m0 + warp + 8 * r) * H + n0 + lane] = v;   // e = tid + r*256 -> (m = e >> 5, n = lane)
-          a.h2t[((size_t)nt * B + m0 + warp + 8 * r) * 32 + lane] = v;   // and the tiled copy [H/32][B][32]
-#pragma unroll
-          for (int o = 0; o < MAXO; ++o) hv_[r * MAXO + o] = v * whr[o];
+          v[r] = fmaxf(outv[r] + b2v, 0.f);
+          a.h2[(size_t)(m0 + warp + 8 * r) * H + n0 + lane] = v[r];   // e = tid + r*256 -> (m = e >> 5, n = lane)
+          a.h2t[((size_t)nt * B + m0 + warp + 8 * r) * 32 + lane] = v[r];   // and the tiled copy [H/32][B][32]
         }
+        // value q = r * MAXO + o is v[r] * whr[o]; the first level pairs q with q + 16 as the products are formed, so
+        // that only 16 values are ever live
+        float hv_[16];
+        const bool up16 = (lane & 16) != 0;
 #pragma unroll
-        for (int off = 16, n = 16; off > 0; off >>= 1, n >>= 1) {
-          const bool up = (lane & off) != 0;
-#pragma unroll
-          for (int q = 0; q < n; ++q) {
-            const float keep = up ? hv_[q + n] : hv_[q], send = up ? hv_[q] : hv_[q + n];
-            hv_[q] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-          }
-        }
+        for (int q = 0; q < 16; ++q) hv_[q] = butterfly_pair(v[q / MAXO] * whr[q % MAXO], v[q / MAXO + 2] * whr[q % MAXO], up16, 16);
+        butterfly_level<8>(hv_, lane);
+        butterfly_level<4>(hv_, lane);
+        butterfly_level<2>(hv_, lane);
+        butterfly_level<1>(hv_, lane);
         TR(35);
         const int r = lane >> 3, o = lane & 7;               // lane l holds value l = r * MAXO + o
         if (o < 4 * nq) a.headp[(((size_t)nt * 2 + (o >> 2)) * B + m0 + warp + 8 * r) * 4 + (o & 3)] = o < nout ? hv_[0] : 0.f;

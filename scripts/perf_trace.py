@@ -59,3 +59,25 @@ for cta in sorted({0, n // 2, n - 1}):
 for a_, b_, nm in [(5, 6, "bar1"), (23, 24, "bar3"), (26, 27, "bar5")]:
     arr = tr[:n, a_] - tr[:n, 0]; dep = tr[:n, b_] - tr[:n, 0]
     print(f"{nm}: arrive min {arr.min()/ghz/1000:.2f} max {arr.max()/ghz/1000:.2f} (cta {arr.argmax()}) | depart-arrive min {(dep - arr).min()/ghz/1000:.2f} us")
+# P1 spans over all CTAs that ran a P1 tile.  A span ends at its slot and starts at the CTA's previous stamped slot of the
+# chain; "row maths" is stamped only by a row tile's last arriver, so the span into bar1 arrival starts at the ticket for the
+# others.  A CTA with several P1 tiles stamps slots 1..37 for its last tile (the earlier ones fall into "h1 generated").
+# g_trace is not cleared between launches and clock64 is per SM, so a slot is used only if it lies inside this CTA's step.
+chain = [(28, "stash issued"), (29, "stash landed"), (1, "h1 generated"), (2, "W2 panel landed"), (3, "mma"),
+         (4, "reduce"), (35, "shuffles"), (36, "ticket"), (37, "row maths (last arrivers)"), (5, "bar1 arrival")]
+us = lambda x: x / ghz / 1000
+p1 = [c for c in range(n) if tr[c, 5] >= tr[c, 1] >= tr[c, 0] > 0]
+spans = {s: [] for s, _ in chain}
+at = {s: [] for s, _ in chain}
+for c in p1:
+    t = tr[c]; prev = t[0]
+    for s, _ in chain:
+        if t[s] < prev or t[s] > t[5]:
+            continue
+        spans[s].append(us(t[s] - prev)); at[s].append(us(t[s] - t[0])); prev = t[s]
+print(f"P1 spans over {len(p1)} CTAs (us; span from the previous slot, @ from the step start)")
+print(f"  {'span end':28s} {'CTAs':>4s} {'median':>7s} {'max':>7s}   {'@median':>7s} {'@max':>7s}")
+for s, nm in chain:
+    if spans[s]:
+        v, w = np.array(spans[s]), np.array(at[s])
+        print(f"  {nm:28s} {len(v):4d} {np.median(v):7.2f} {v.max():7.2f}   {np.median(w):7.2f} {w.max():7.2f}")
