@@ -277,31 +277,39 @@ template <bool A_KC>
 __device__ __forceinline__ int tile_row(int ty, int i) { return A_KC ? (ty + 4 * i) : (ty * 8 + i); }
 
 // fold the 16 k-groups in a fixed order; thread gets outputs e = tid + r*256 -> (m = e>>5, n = e&31).
-// The caller has synchronised the CTA since the last read of the memory behind `red` (RED_FLOATS).
-// Element (i, j) of thread (ty, tx) always goes to slot (ty + 4 i, tx + 4 j) of its group's 32 x 36 block,
-// whatever tile row / column it stands for: the 32 lanes of a store then hit 32 distinct banks (group blocks
-// are 16 banks apart).  The reader maps its output (m, n) back through the panel's row order.
+// The caller has synchronised the CTA since the last read of the memory behind `red` (RED_FLOATS), and synchronises
+// it again before anyone writes there (no trailing barrier here: P1's next writer is already behind the ticket's).
+// Row i of thread (ty, tx) always goes to row slot ty + 4 i of its group's 32 x 36 block and its 8 elements to column
+// slots 8 tx .. 8 tx + 7, whatever tile row / columns they stand for: two 16-byte stores per row, and the 8 lanes of a
+// quarter-warp phase (tx = 0..3, two ty) cover 32 distinct banks (group blocks are 16 banks apart).  The reader maps
+// its output (m, n) back through the panels' row / column orders; a warp reads one row slot, 32 distinct banks.
 constexpr int RED_GS = 32 * 36 + 16;
 template <bool KC>
-__device__ __forceinline__ int red_slot(int idx) { return KC ? idx : ((idx >> 3) + 4 * (idx & 7)); }
+__device__ __forceinline__ int red_row(int m) { return KC ? m : ((m >> 3) + 4 * (m & 7)); }
+template <bool KC>
+__device__ __forceinline__ int red_col(int n) { return KC ? (8 * (n & 3) + (n >> 2)) : n; }
 template <bool A_KC, bool B_KC>
 __device__ __forceinline__ void tile_reduce(const float (&acc)[8][8], float* red, float (&outv)[4]) {
   const int tid = threadIdx.x, grp = tid >> 4, t = tid & 15, tx = t & 3, ty = t >> 2;
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) red[grp * RED_GS + (ty + 4 * i) * 36 + tx + 4 * j] = acc[i][j];
+  for (int i = 0; i < 8; ++i) {
+    float4* p = reinterpret_cast<float4*>(&red[grp * RED_GS + (ty + 4 * i) * 36 + 8 * tx]);
+    p[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+    p[1] = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+  }
   __syncthreads();
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     const int e = tid + r * NT, m = e >> 5, n = e & 31;
-    const int off = red_slot<A_KC>(m) * 36 + red_slot<B_KC>(n);
+    const int off = red_row<A_KC>(m) * 36 + red_col<B_KC>(n);
+    float g_[KG];
+#pragma unroll
+    for (int g = 0; g < KG; ++g) g_[g] = red[g * RED_GS + off];
     float v = 0.f;
 #pragma unroll
-    for (int g = 0; g < KG; ++g) v += red[g * RED_GS + off];
+    for (int g = 0; g < KG; ++g) v += g_[g];
     outv[r] = v;
   }
-  __syncthreads();
 }
 
 // fixed-order block sum of one float (all threads call; every thread gets the result)
@@ -330,14 +338,19 @@ __device__ __forceinline__ void butterfly_level(float (&h)[S], int lane) {
   for (int q = 0; q < N; ++q) h[q] = butterfly_pair(h[q], h[q + N], up, N);
 }
 
-// d (loss) / d (h2 pre-activation) for 4 adjacent columns of one row: (dout[row] . Wh[:, c..c+3]) * relu'(h2)
+// d (loss) / d (h2 pre-activation) for 4 adjacent columns of one row: (dout[row] . Wh[:, c..c+3]) * relu'(h2).
+// MO >= nout bounds the head outputs: dout and wr are zero beyond nout, and each term left out would be fmaf(0, 0, t),
+// which returns t (the sum of +0 and a zero t is +0 where t = -0; the relu mask, the tile products and the squares of
+// the norm do not tell the two zeros apart).
+template <int MO>
 __device__ __forceinline__ float4 dh2_quad(const float* drow, const float4 (&wr)[MAXO], float4 hv) {
+  static_assert(MO >= 1 && MO <= MAXO, "head output bound");
   const float4 d0 = *reinterpret_cast<const float4*>(drow);
   const float4 d1 = *reinterpret_cast<const float4*>(drow + 4);
   const float d[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
   float4 t = make_float4(d[0] * wr[0].x, d[0] * wr[0].y, d[0] * wr[0].z, d[0] * wr[0].w);
 #pragma unroll
-  for (int o = 1; o < MAXO; ++o) {
+  for (int o = 1; o < MO; ++o) {
     t.x = fmaf(d[o], wr[o].x, t.x); t.y = fmaf(d[o], wr[o].y, t.y); t.z = fmaf(d[o], wr[o].z, t.z); t.w = fmaf(d[o], wr[o].w, t.w);
   }
   return make_float4(hv.x > 0.f ? t.x : 0.f, hv.y > 0.f ? t.y : 0.f, hv.z > 0.f ? t.z : 0.f, hv.w > 0.f ? t.w : 0.f);
@@ -428,6 +441,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
   const int cta = blockIdx.x;
   const int B = a.B, D = a.D, H = a.H, A = a.A, nout = a.nout;
   const int npol = a.continuous ? 2 * A : A;
+  constexpr int NO = 2 * NA + 1 < MAXO ? 2 * NA + 1 : MAXO;   // >= nout = npol + 1 (the host picks NA >= A)
   const int nq = (nout + 3) >> 2;              // float4 quads of head outputs per row
   const float invB = 1.0f / (float)B;
   const jbppo::HP hp{a.eps_clip, a.vf_coef, a.ent_coef};
@@ -1045,7 +1059,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           for (int o = 0; o < MAXO; ++o) wr[o] = o < nout ? *reinterpret_cast<const float4*>(&PS[o * PK + nc * 32 + 4 * c8]) : make_float4(0.f, 0.f, 0.f, 0.f);
           const float4 hcur = hq;
           if (nc + 1 < NKC) hq = ldcg4(a.h2 + (size_t)(m0 + ml) * H + (nc + 1) * 32 + 4 * c8);
-          const float4 dv = dh2_quad(drow, wr, hcur);
+          const float4 dv = dh2_quad<NO>(drow, wr, hcur);
           const float4 lo = make_float4(tf32_lo(dv.x), tf32_lo(dv.y), tf32_lo(dv.z), tf32_lo(dv.w));
           const unsigned bbuf = tc_base + TC_NA * TC_A_BYTES + slot * TC_B_BYTES, off = tile_off(ml, c8);
           asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"r"(bbuf + off), "f"(dv.x), "f"(dv.y), "f"(dv.z), "f"(dv.w) : "memory");
@@ -1135,7 +1149,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           for (int r = 0; r < 16; ++r) {
             const int row = rh * 16 + r;
             float4* pa = reinterpret_cast<float4*>(&R0[row * (H + 4) + c4]);
-            *pa = dh2_quad(&dsm[(m0 + row) * MAXO], wr, *pa);
+            *pa = dh2_quad<NO>(&dsm[(m0 + row) * MAXO], wr, *pa);
           }
         }
         __syncthreads();
@@ -1160,6 +1174,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           for (int i = 0; i < MAXD; ++i) if (i < D) wacc[i] = fmaf(dv, xrow[i * 32], wacc[i]);
           wacc[MAXD] += dv;
         }
+        __syncthreads();                           // the fold's reads of R0 are done
 #pragma unroll
         for (int i = 0; i <= MAXD; ++i) if (i < D || i == MAXD) R0[(warp * (MAXD + 1) + i) * 32 + lane] = wacc[i];
         __syncthreads();
@@ -1321,7 +1336,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
               TR(17);
               for (int m = rl; m < kp; m += 32) {
                 float4* pa = reinterpret_cast<float4*>(&R2[m * 32 + 4 * cg]);
-                *pa = dh2_quad(&dsm[(mp + m) * MAXO], wr, *pa);
+                *pa = dh2_quad<NO>(&dsm[(mp + m) * MAXO], wr, *pa);
               }
               __syncthreads();
               TR(18);
@@ -1341,6 +1356,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           }
           if (kt == 0) {
             const int grp = tid >> 4, t = tid & 15, tx = t & 3, ty = t >> 2;
+            __syncthreads();                       // the fold's reads of R0 are done
             if (tx == 0) {
 #pragma unroll
               for (int i = 0; i < 8; ++i) R0[grp * 32 + ty * 8 + i] = rs[i];
@@ -1368,6 +1384,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           const int kp = min(JA_ROWS, B - mp);
           if (!(mp == 0 && pre_job == job)) { __syncthreads(); stage_block(st, R2, a.h2t + ((size_t)jt * B + mp) * 32, kp); st.commit(); }
           st.wait();
+          if (!TC) TR(39);                 // (JC / JD stamps: FFMA engine only, they cost the tensor-core instantiations spills)
 #pragma unroll 4
           for (int m = warp; m < kp; m += NT / 32) {
             const float hvv = R2[m * 32 + lane];
@@ -1409,6 +1426,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
             if (tid < nout) { *ht.gb[tid] = tt; sq = fmaf(tt, tt, sq); }
           }
         }
+        if (!TC) TR(30);
       } else {
         // ---- dW1 / db1 of 32 hidden units: fixed-order fold of the MT tile partials ----------------------
         const int kt = job - nJB - nJA - nJC, k0 = kt * 32;
@@ -1421,6 +1439,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           asm volatile("fence.acq_rel.gpu;\n" ::: "memory");
         }
         __syncthreads();
+        if (!TC) TR(31);
         for (int e = tid; e < 32 * (D + 1); e += NT) {
           const int n = e / (D + 1), i = e - n * (D + 1);
           float t = ldcg(a.w1p + (size_t)k0 * (D + 1) + e);
@@ -1428,6 +1447,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_epoch_kernel(Args a, int dsm_floats
           if (i < D) a.gW1[(size_t)(k0 + n) * D + i] = t; else a.gb1[k0 + n] = t;
           sq = fmaf(t, t, sq);
         }
+        if (!TC) TR(32);
       }
     }
     TR(22);
