@@ -375,4 +375,39 @@ JB_API int jb_munchausen_quantile_loss(const float* pred, const float* next_targ
                                        const float* done, int B, int A, int N, int Np, int Nc, float gamma, float m_alpha,
                                        float m_tau, float l0, float* dpred, float* stats, float* scratch, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * R2D2 (Kapturowski et al., ICLR 2019): a recurrent dueling Q-network on replayed sequences, csrc/lstm.cu and csrc/r2d2.cu.
+ * The LSTM uses torch.nn.LSTM's layout and gate order i, f, g, o (weight_hh [4H, H]); the caller forms the input
+ * projection of all time steps at once, xg = x W_ih^T + b_ih + b_hh [rows, 4H], with jb_linear_fwd.
+ *   jb_lstm_step_fwd   one step over M rows: i, f, o = sigm(xg + h_prev W_hh^T), g = tanh(.), c = f c_prev + i g,
+ *                      h = o tanh(c); gates [M, 4H] receives the post-activation (i, f, g, o).  reset [M] (may be NULL):
+ *                      rows with reset != 0 read h_prev and c_prev as zero (an episode starts at this step).  hprev_eff
+ *                      (may be NULL) receives h_prev with those rows zeroed, the operand of dW_hh.  c may alias c_prev;
+ *                      h and hprev_eff must not alias h_prev.
+ *   jb_lstm_step_bwd   dh = dh_out + (dgates_next W_hh) and dcell = dh o (1 - tanh^2 c) + dc_next, where the two recurrent
+ *                      terms are dropped on rows with reset_next != 0 (the next step did not read this step's state);
+ *                      dgates [M, 4H] = d loss / d (i, f, g, o pre-activations), with c_prev read as zero where reset != 0;
+ *                      dc [M, H] (may be NULL, may alias dc_next) = dcell f, the gradient into the c_prev this step read.
+ *                      dh_out, dgates_next, dc_next, reset, reset_next may be NULL (zero / no reset).
+ *                      A CTA owns 8 hidden units and 32 rows; fp32 FFMA in ascending k, no atomics: bit-reproducible.
+ *   jb_r2d2_loss       q, q_next (online on s, s'), qt_next (target on s') [B, T, A]; action int64 [B, T];
+ *                      reward / done [B, T + n_step] (step t uses columns t .. t + n_step - 1); weights f64 [B] or NULL;
+ *                      a* = argmax_a q_next[b, t, a] (first index on ties);
+ *                      y = h(fold_{i = n-1 .. 0} (r_{t+i} + (1 - d_{t+i}) gamma y)) from y = h^-1(qt_next[b, t, a*]),
+ *                      h(x) = sign(x)(sqrt(|x| + 1) - 1) + 1e-3 x;  td = y - q[b, t, a_t];
+ *                      loss = (1/(B T)) sum_b sum_t w_b td^2, dq = its gradient (on the taken action only, 0 elsewhere);
+ *                      prio [B] (f64, may be NULL) = (eta max_t |td| + (1 - eta) mean_t |td|)^alpha from the unweighted td;
+ *                      stats = {loss, max_{b,t} q[b, t, a_t]}; scratch: 2*B doubles.  Targets and sums in float64.
+ *                      1 <= A <= 18, n_step >= 1, B, T >= 1, else JB_ERR_INVALID.  One CTA per sequence, fixed-order
+ *                      sums and a single-thread finalize: bit-reproducible.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_lstm_step_fwd(const float* xg, const float* h_prev, const float* c_prev, const float* w_hh, const float* reset,
+                            int M, int H, float* h, float* c, float* gates, float* hprev_eff, void* stream);
+JB_API int jb_lstm_step_bwd(const float* dh_out, const float* dgates_next, const float* w_hh, const float* gates,
+                            const float* c_prev, const float* c, const float* dc_next, const float* reset,
+                            const float* reset_next, int M, int H, float* dgates, float* dc, void* stream);
+JB_API int jb_r2d2_loss(const float* q, const float* q_next, const float* qt_next, const int64_t* action, const float* reward,
+                        const float* done, const double* weights, int B, int T, int A, int n_step, float gamma, float alpha,
+                        float eta, float* dq, double* prio, float* stats, double* scratch, void* stream);
+
 #endif /* JORLDY_B200_H */

@@ -3,7 +3,7 @@
 `load("config.<agent>.<env>")` returns a module-like namespace with the four dicts the reference's
 config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / train).  Values follow the
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
-per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
+per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, r2d2, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
@@ -79,6 +79,25 @@ def _ape_x_config(env):
     env_d = dict(name="cartpole", action_type="discrete", render=False) if env == "cartpole" else dict(name="mountain_car", render=False)
     return dict(env=env_d, agent=a, optim=dict(opt, lr=1e-4),
                 train=dict(_TRAIN_SMALL, eval_iteration=10, distributed_batch_size=512, update_period=16, num_workers=32))
+
+
+def _r2d2_config(env):
+    """R2D2 (Kapturowski et al., ICLR 2019).  atari: the paper's Table 2 (gamma 0.997, n 5, sequences of 80 with a burn-in
+    of 40 stored every 40 steps, batch 64, Adam lr 1e-4 eps 1e-3, target period 2500, alpha 0.9, beta 0.6, eta 0.9, LSTM
+    512, gradient clip 40), a replay of 100 000 sequences (4 M observations at stride 40) and Ape-X's actor epsilons.
+    cartpole / mountaincar: Ape-X's row with seq_len 16, n_burn_in 8, n_step 4, eta 0.9, a choice of this project.  Not
+    compared with the reference's config/r2d2/*.py, which takes precedence when a JORLDY config directory is on
+    sys.path."""
+    keys = dict(name="r2d2", network="r2d2", eta=0.9, zero_padding=True)
+    if env == "atari":
+        a = dict(keys, head="cnn", gamma=0.997, n_step=5, seq_len=80, n_burn_in=40, batch_size=64, buffer_size=100000,
+                 start_train_step=50000, target_update_period=2500, alpha=0.9, beta=0.6, uniform_sample_prob=1e-3,
+                 hidden_size=512, clip_grad_norm=40.0, lr_decay=True)
+        return dict(env=dict(_ATARI_ENV), agent=a, optim=dict(name="adam", lr=1e-4, eps=1e-3),
+                    train=dict(_TRAIN_ATARI, update_period=100, num_workers=128))
+    d = _ape_x_config(env)
+    d["agent"].update(keys, seq_len=16, n_burn_in=8, n_step=4)
+    return d
 
 
 def _ppo_config(env):
@@ -179,7 +198,7 @@ def available():
     for ag, envs in _AC_ENVS.items():
         out += [f"config.{ag}.{e}" for e in envs]
     out += [f"config.sac_discrete.{e}" for e in ("cartpole", "atari")]
-    for ag in list(_VALUE_AGENTS) + ["ape_x"]:
+    for ag in list(_VALUE_AGENTS) + ["ape_x", "r2d2"]:
         out += [f"config.{ag}.{e}" for e in ("cartpole", "mountaincar", "atari")]
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
     return out
@@ -194,6 +213,8 @@ def load(config_path):
         d = _value_config(agent, env)
     elif agent == "ape_x" and env in ("cartpole", "mountaincar", "atari"):
         d = _ape_x_config(env)
+    elif agent == "r2d2" and env in ("cartpole", "mountaincar", "atari"):
+        d = _r2d2_config(env)
     elif agent == "ppo" and env in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari"):
         d = _ppo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:

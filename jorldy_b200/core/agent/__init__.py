@@ -7,9 +7,10 @@ from .ddpg import DDPG, TD3, SAC
 from .quantile import IQN, QRDQN
 from .munchausen import MDQN, MIQN
 from .rainbow_iqn import RainbowIQN
+from .r2d2 import R2D2
 
 agent_dict = OrderedDict(sorted(dict(ape_x=ApeX, c51=C51, ddpg=DDPG, double=Double, dqn=DQN, dueling=Dueling, iqn=IQN,
-                                     m_dqn=MDQN, m_iqn=MIQN, multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, qrdqn=QRDQN,
+                                     m_dqn=MDQN, m_iqn=MIQN, multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, qrdqn=QRDQN, r2d2=R2D2,
                                      rainbow=Rainbow, rainbow_iqn=RainbowIQN, sac=SAC, td3=TD3).items()))
 
 

@@ -113,6 +113,51 @@ class NStepAssembler:
         return out
 
 
+class SequenceAssembler:
+    """Device-side assembly of R2D2's replayed sequences for N batched lanes (Kapturowski et al., ICLR 2019).
+
+    Each lane keeps a ring of L = n_burn_in + seq_len + n_step steps.  Once L steps have been pushed, the N windows of the
+    last L steps are emitted every store_period = seq_len // 2 steps (windows overlap by L - store_period steps).  Like
+    NStepAssembler's windows, they are not cut at episode ends: `reset` marks the steps that start an episode, and the
+    learner's unroll zeroes the recurrent state there, exactly where the actor did.
+
+    push(tr) takes the step's fields, each with leading dim N: state (or int64 frame references), action, prev_action
+    (-1 at an episode's first step), reset (f32), reward, done, and, at the steps where starts_window() is true, the
+    actor's (h0, c0) from before the step.  Only those snapshots are kept (at most ceil(L / store_period) + 1 of them),
+    never an [N, L, H] history.  An emitted window holds every field as [N, L, ...] oldest step first, plus h0 / c0 [N, H]
+    of its first step.
+    """
+
+    FIELDS = ("state", "action", "prev_action", "reset", "reward", "done")
+
+    def __init__(self, n_burn_in, seq_len, n_step):
+        self.L = int(n_burn_in) + int(seq_len) + int(n_step)
+        self.period = max(1, int(seq_len) // 2)
+        self.hist, self.t, self.pos, self.snap = None, 0, 0, {}
+
+    def starts_window(self):
+        """True if the next pushed step is the first step of a window (its pre-step (h, c) must come with it)."""
+        return self.t % self.period == 0
+
+    def push(self, tr):
+        if self.hist is None:
+            self.hist = {k: torch.zeros((tr[k].shape[0], self.L) + tuple(tr[k].shape[1:]), dtype=tr[k].dtype,
+                                        device=tr[k].device) for k in self.FIELDS}
+        if self.starts_window():
+            self.snap[self.t] = (tr["h0"].clone(), tr["c0"].clone())
+        for k in self.FIELDS:
+            self.hist[k][:, self.pos].copy_(tr[k])
+        self.pos = (self.pos + 1) % self.L
+        self.t += 1
+        start = self.t - self.L
+        if start < 0 or start % self.period:
+            return None
+        sel = torch.as_tensor([(self.pos + i) % self.L for i in range(self.L)], device=self.hist["reward"].device)
+        out = {k: v.index_select(1, sel) for k, v in self.hist.items()}
+        out["h0"], out["c0"] = self.snap.pop(start)
+        return out
+
+
 class ReplayCollector:
     """Off-policy resident loop: `update_period` batched env steps feeding the HBM replay, then one
     agent.process() (the reference's sync loop, run_mode.py:180-187: one learn per round whatever the
@@ -122,12 +167,17 @@ class ReplayCollector:
         self.env, self.agent, self.update_period = env, agent, update_period
         n = getattr(agent, "n_step", 1)
         apex = type(agent).__name__ == "ApeX"
-        self.assembler = NStepAssembler(n, apex, agent.gamma) if (n > 1 or apex) else None
-        if apex:
+        # recurrent agents (R2D2) bring their own sequence assembler and frame store
+        self.sequences = getattr(agent, "sequence_assembler", None)
+        self.assembler = NStepAssembler(n, apex, agent.gamma) if (n > 1 or apex) and self.sequences is None else None
+        if apex or self.sequences is not None:
             agent.set_actor_epsilons(env.num_envs, total=max(agent.num_workers, env.num_envs, 2))
         env.reset_device()
         # Atari-shaped envs: every frame is pushed once and the replay stores frame references (buffer/frame_store.py)
-        self.frames = frame_store.attach(env, agent.memory, n)
+        if self.sequences is not None:
+            self.frames = agent.attach_frames(env)
+        else:
+            self.frames = frame_store.attach(env, agent.memory, n)
         if self.frames is not None:
             self.frames.start(env.obs)
 
@@ -142,6 +192,14 @@ class ReplayCollector:
                 state, next_state = self.frames.push(env.obs, next_obs, done, env.auto_reset)
             else:
                 next_state = next_obs.clone()
+            if self.sequences is not None:
+                tr = dict(agent.step_inputs, state=state, action=action.clone(), reward=reward.view(-1).clone(),
+                          done=done.view(-1).clone())
+                agent.end_step(tr["done"])
+                out = self.sequences.push(tr)
+                if out is not None:
+                    batches.append(out)
+                continue
             tr = {"state": state, "action": action.view(action.shape[0], -1).clone(), "reward": reward.clone(), "done": done.clone(),
                   "next_state": next_state}
             if self.assembler is not None:

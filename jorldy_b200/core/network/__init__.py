@@ -8,6 +8,7 @@ from .iqn import IQN
 from .noisy import Noisy, Rainbow
 from .policy import ContinuousPolicy, DeterministicPolicy, DiscretePolicy
 from .q_network import ContinuousQ_Network
+from .r2d2 import R2D2
 from .rainbow_iqn import RainbowIQN
 
 network_dict = OrderedDict(
@@ -21,6 +22,7 @@ network_dict = OrderedDict(
     dueling=Dueling,
     iqn=IQN,
     noisy=Noisy,
+    r2d2=R2D2,
     rainbow=Rainbow,
     rainbow_iqn=RainbowIQN,
 )
