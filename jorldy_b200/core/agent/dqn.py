@@ -30,6 +30,7 @@ class DQN(BaseAgent):
     _loss_kind = 0      # 0 smooth_l1, 1 IS-weighted MSE
     _order = 0          # 0 dqn.py product order, 1 double.py/per.py order, 2 n-step loop
     _clip = None
+    _decay_eps = True   # process() decays epsilon once learning has started (not the noisy agents, nor Ape-X's fixed ones)
 
     def __init__(self, state_size, action_size, hidden_size=512, optim_config={"name": "adam"},
                  network="discrete_q_network", head="mlp", gamma=0.99, epsilon_init=1.0, epsilon_min=0.1,
@@ -80,6 +81,13 @@ class DQN(BaseAgent):
         self.network.forward_rows(state, q)
         return q
 
+    def _warmup_actions(self, M, training):
+        """Uniform random actions for M rows while the replay holds fewer than max(batch_size, start_train_step)
+        transitions (noisy.py:71-72, rainbow.py:143-147); None once past that or when not training."""
+        if training and self.memory.size < max(self.batch_size, self.start_train_step):
+            return torch.randint(0, self.action_size, (M,), device=self.device)
+        return None
+
     def act_device(self, state, training=True, noise=None):
         """state [N, ...] device tensor -> (action int64 [N], q_sel f32 [N])."""
         M = state.shape[0]
@@ -127,17 +135,31 @@ class DQN(BaseAgent):
     def _forward_q(self, net, x, tag, is_train=True, noise=None):
         return net.forward(x, tag=tag)
 
-    def _learn_batch(self, batch, weights=None):
-        """Shared TD learner. batch: device tensors state, action, reward [B,n], done [B,n], next_state."""
+    def _batch_tensors(self, batch, n=-1):
+        """A replay batch as the loss kernels read it: (B, state, next_state, reward f32 [B, n], done f32 [B, n],
+        action [B] int64 / int32 / float32, other dtypes as int64).  The single-step losses pass n = 1, so that a batch
+        of n-step windows fails here instead of being read as one step."""
         B = batch["reward"].shape[0]
-        A = self.action_size
         state = self._net_input(batch["state"])
         next_state = self._net_input(batch["next_state"])
-        reward = batch["reward"].to(torch.float32).reshape(B, -1).contiguous()
-        done = batch["done"].to(torch.float32).reshape(B, -1).contiguous()
+        reward = batch["reward"].to(torch.float32).reshape(B, n).contiguous()
+        done = batch["done"].to(torch.float32).reshape(B, n).contiguous()
         action = batch["action"].reshape(B).contiguous()
         if action.dtype not in (torch.int64, torch.int32, torch.float32):
             action = action.to(torch.int64)
+        return B, state, next_state, reward, done, action
+
+    def _optimizer_step(self):
+        """After the backward: the allreduce hook on the flat gradient, then the (clipped) optimizer step."""
+        if self.allreduce is not None:
+            self.allreduce(self.network.grad)
+        self.optimizer.step(max_norm=self._clip)
+        self.num_learn += 1
+
+    def _learn_batch(self, batch, weights=None):
+        """Shared TD learner. batch: device tensors state, action, reward [B,n], done [B,n], next_state."""
+        B, state, next_state, reward, done, action = self._batch_tensors(batch)
+        A = self.action_size
         net, tgt = self.network, self.target_network
         noise = getattr(self, "_inject_noise", None) or [None, None, None]
         q = self._forward_q(net, state, "t.", True, noise[0])
@@ -149,10 +171,7 @@ class DQN(BaseAgent):
                      ptr(weights), B, A, self.gamma, float(self.alpha), reward.shape[1], self._double_q, self._loss_kind,
                      self._order, ptr(dq), ptr(prio), ptr(self._stats), stream_ptr())
         net.backward(dq, B, tag="t.")
-        if self.allreduce is not None:
-            self.allreduce(net.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
+        self._optimizer_step()
         return prio
 
     def learn(self):
@@ -176,7 +195,8 @@ class DQN(BaseAgent):
             if self.lr_decay:
                 self.learning_rate_decay(step)
         if self.num_learn > 0:
-            self.epsilon_decay(delta_t)
+            if self._decay_eps:
+                self.epsilon_decay(delta_t)
             if self.target_update_stamp >= self.target_update_period:
                 self.update_target()
                 self.target_update_stamp -= self.target_update_period
@@ -223,23 +243,6 @@ class Multistep(DQN):
         self.n_step = n_step
         self.tmp_buffer = deque(maxlen=n_step)
 
-    def process(self, transitions, step):
-        result = {}
-        delta_t = step - self.time_t
-        self.memory.store(transitions)
-        self.time_t = step
-        self.target_update_stamp += delta_t
-        if self.memory.size >= self.batch_size and self.time_t >= self.start_train_step:
-            result = self.learn()
-            if self.lr_decay:
-                self.learning_rate_decay(step)
-        if self.num_learn > 0:
-            self.epsilon_decay(delta_t)
-            if self.target_update_stamp >= self.target_update_period:
-                self.update_target()
-                self.target_update_stamp -= self.target_update_period
-        return result
-
     def interact_callback(self, transition):
         return _nstep_callback(self, transition)
 
@@ -277,7 +280,7 @@ class PER(DQN):
         return {"loss": loss, "epsilon": self.epsilon, "beta": self.beta, "max_Q": max_q, "sampled_p": sampled_p,
                 "mean_p": mean_p}
 
-    def _stamped_process(self, transitions, step, counter_attr, decay_eps):
+    def _stamped_process(self, transitions, step, counter_attr):
         """per.py:90-122 / rainbow.py:255-283 / ape_x.py:135-164: learn at most once per call while the
         learn-period stamp has backlog."""
         result = {}
@@ -295,7 +298,7 @@ class PER(DQN):
                 self.learning_rate_decay(step)
             self.learn_period_stamp -= self.learn_period
         if self.num_learn > 0:
-            if decay_eps:
+            if self._decay_eps:
                 self.epsilon_decay(delta_t)
             if self.target_update_stamp >= self.target_update_period:
                 self.update_target()
@@ -303,10 +306,12 @@ class PER(DQN):
         return result
 
     def process(self, transitions, step):
-        return self._stamped_process(transitions, step, "size", True)
+        return self._stamped_process(transitions, step, "size")
 
 
 class Noisy(DQN):
+    _decay_eps = False
+
     def __init__(self, state_size, action_size, hidden_size=512, network="noisy", head="mlp", noise_type="factorized",
                  **kwargs):
         self._noise_type = noise_type
@@ -328,9 +333,8 @@ class Noisy(DQN):
 
     def act_device(self, state, training=True, noise=None):
         """noise: injected NoisyNet draws [(eps_i, eps_j)] x 2 for this forward (parity tests)."""
-        M = state.shape[0]
-        if training and self.memory.size < max(self.batch_size, self.start_train_step):
-            action = torch.randint(0, self.action_size, (M,), device=self.device)      # noisy.py:71-72
+        action = self._warmup_actions(state.shape[0], training)
+        if action is not None:
             return action, None
         q = self._q_values(state, training, noise=noise)
         return torch.argmax(q, -1), None
@@ -343,21 +347,6 @@ class Noisy(DQN):
         s1, s2 = self.network.get_sig_w_mean()
         return {"loss": float(st[0]), "max_Q": float(st[1]), "sig_w1": float(s1.item()), "sig_w2": float(s2.item())}
 
-    def process(self, transitions, step):
-        result = {}
-        self.memory.store(transitions)
-        delta_t = step - self.time_t
-        self.time_t = step
-        self.target_update_stamp += delta_t
-        if self.memory.size >= self.batch_size and self.time_t >= self.start_train_step:
-            result = self.learn()
-            if self.lr_decay:
-                self.learning_rate_decay(step)
-        if self.num_learn > 0 and self.target_update_stamp >= self.target_update_period:
-            self.update_target()
-            self.target_update_stamp -= self.target_update_period
-        return result
-
 
 class _Distributional:
     """C51 machinery shared by C51 and Rainbow (support z, fused projection/KL kernel)."""
@@ -368,13 +357,8 @@ class _Distributional:
         self.z = torch.linspace(v_min, v_max, num_support, device=self.device).view(1, -1)
 
     def _dist_learn(self, batch, weights, variant, noise):
-        B = batch["reward"].shape[0]
+        B, state, next_state, reward, done, action = self._batch_tensors(batch)
         A, K = self.action_size, self.num_support
-        state = self._net_input(batch["state"])
-        next_state = self._net_input(batch["next_state"])
-        reward = batch["reward"].to(torch.float32).reshape(B, -1).contiguous()
-        done = batch["done"].to(torch.float32).reshape(B, -1).contiguous()
-        action = batch["action"].reshape(B).contiguous()
         net, tgt = self.network, self.target_network
         logits = self._forward_logits(net, state, "t.", noise[0])
         next_online = self._forward_logits(net, next_state, "n.", noise[1]) if variant == 1 else None
@@ -388,10 +372,7 @@ class _Distributional:
                       float(self.alpha), reward.shape[1], variant, ptr(dlogits), ptr(kl), ptr(prio), ptr(self._stats),
                       ptr(scratch), stream_ptr())
         net.backward(dlogits.view(B, A * K), B, tag="t.")
-        if self.allreduce is not None:
-            self.allreduce(net.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
+        self._optimizer_step()
         return prio
 
     def _expected_q(self, logits, M):
@@ -426,6 +407,8 @@ class C51(DQN, _Distributional):
 
 
 class Rainbow(PER, _Distributional):
+    _decay_eps = False
+
     def __init__(self, state_size, action_size, hidden_size=512, network="rainbow", head="mlp",
                  optim_config={"name": "adam"}, gamma=0.99, buffer_size=50000, batch_size=64, start_train_step=2000,
                  target_update_period=500, run_step=1e6, lr_decay=True, n_step=4, alpha=0.6, beta=0.4, learn_period=4,
@@ -454,16 +437,19 @@ class Rainbow(PER, _Distributional):
         """One noisy forward for all rows (the reference's act() with a batch of N states draws its noise once per
         call, rainbow.py:149).  noise: injected draws [(eps_i, eps_j)] x 4 in call order a1, v1, a2, v2."""
         M = state.shape[0]
-        if training and self.memory.size < max(self.batch_size, self.start_train_step):
-            return torch.randint(0, self.action_size, (M,), device=self.device), None       # rainbow.py:143-147
+        action = self._warmup_actions(M, training)
+        if action is not None:
+            return action, None
         logits = self.network._buf("act.logits", (M, self.action_size, self.num_support))
         self.network.forward_rows(state, logits, is_train=training, noise=noise)
         return torch.argmax(self._expected_q(logits, M), -1), None
 
+    def _learn_batch(self, batch, weights=None):
+        return self._dist_learn(batch, weights, 1, self._inject_noise or [None, None, None])
+
     def learn(self):
         batch, weights, indices, stats_per = self._per_sample()
-        noise = self._inject_noise or [None, None, None]
-        prio = self._dist_learn(batch, weights, 1, noise)
+        prio = self._learn_batch(batch, weights)
         self.memory.update_priorities(indices, prio)
         st = self._stats.cpu().numpy()
         sp = stats_per.cpu().numpy()
@@ -472,7 +458,7 @@ class Rainbow(PER, _Distributional):
                 "min_logit": float(st[3]), "sampled_p": float(sp[0]), "mean_p": float(sp[1])}
 
     def process(self, transitions, step):
-        return self._stamped_process(transitions, step, "counter", False)
+        return self._stamped_process(transitions, step, "counter")
 
     def interact_callback(self, transition):
         return _nstep_callback(self, transition)
@@ -480,6 +466,7 @@ class Rainbow(PER, _Distributional):
 
 class ApeX(PER):
     _double_q, _loss_kind, _order = 1, 1, 2
+    _decay_eps = False
 
     def __init__(self, epsilon=0.4, epsilon_alpha=7.0, clip_grad_norm=40.0, alpha=0.6, beta=0.4, learn_period=4,
                  uniform_sample_prob=1e-3, n_step=4, **kwargs):
@@ -510,7 +497,7 @@ class ApeX(PER):
 
     def process(self, transitions, step):
         self.num_transitions += sum(int(np.shape(t["reward"])[0]) for t in transitions)
-        return self._stamped_process(transitions, step, "counter", False)
+        return self._stamped_process(transitions, step, "counter")
 
     def set_distributed(self, id):
         assert self.num_workers > 1

@@ -13,22 +13,9 @@ M-IQN draws three fraction sets per learn from IQN's Philox stream, in this orde
 tau'(s') for the target pass on s', tau''(s) for the target pass on s (tests inject them as _inject_tau[0], [1], [3];
 [2] is act()'s).
 """
-import torch
-
 from ..dev import C, ptr, stream_ptr
 from .dqn import DQN, _action_kind
 from .quantile import IQN
-
-
-def _batch_tensors(agent, batch):
-    B = batch["reward"].shape[0]
-    state, next_state = agent._net_input(batch["state"]), agent._net_input(batch["next_state"])
-    reward = batch["reward"].to(torch.float32).reshape(B).contiguous()
-    done = batch["done"].to(torch.float32).reshape(B).contiguous()
-    action = batch["action"].reshape(B).contiguous()
-    if action.dtype not in (torch.int64, torch.int32, torch.float32):
-        action = action.to(torch.int64)
-    return B, state, next_state, reward, done, action
 
 
 class _Munchausen:
@@ -37,12 +24,6 @@ class _Munchausen:
             raise ValueError(f"Munchausen RL needs tau > 0 and l_0 <= 0 (got tau={tau}, l_0={l_0})")
         self.m_alpha, self.m_tau, self.m_l0 = float(alpha), float(tau), float(l_0)
 
-    def _finish_step(self):
-        if self.allreduce is not None:
-            self.allreduce(self.network.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
-
 
 class MDQN(_Munchausen, DQN):
     def __init__(self, state_size, action_size, alpha=0.9, tau=0.03, l_0=-1, **kwargs):
@@ -50,7 +31,7 @@ class MDQN(_Munchausen, DQN):
         self._set_munchausen(alpha, tau, l_0)
 
     def _learn_batch(self, batch, weights=None):
-        B, state, next_state, reward, done, action = _batch_tensors(self, batch)
+        B, state, next_state, reward, done, action = self._batch_tensors(batch, 1)
         A, net, tgt = self.action_size, self.network, self.target_network
         q = net.forward(state, tag="t.")
         qt_next = tgt.forward(next_state, tag="n.")
@@ -61,7 +42,7 @@ class MDQN(_Munchausen, DQN):
                        self.gamma, self.m_alpha, self.m_tau, self.m_l0, ptr(dq), ptr(self._stats), ptr(scratch),
                        stream_ptr())
         net.backward(dq, B, tag="t.")
-        self._finish_step()
+        self._optimizer_step()
 
 
 class MIQN(_Munchausen, IQN):
@@ -70,7 +51,7 @@ class MIQN(_Munchausen, IQN):
         self._set_munchausen(alpha, tau, l_0)
 
     def _learn_batch(self, batch, weights=None):
-        B, state, next_state, reward, done, action = _batch_tensors(self, batch)
+        B, state, next_state, reward, done, action = self._batch_tensors(batch, 1)
         A, N, net, tgt = self.action_size, self.num_sample, self.network, self.target_network
         tau = self._draw_tau(B, 0.0, 1.0, "t.tau", 0)
         tau_next = self._draw_tau(B, 0.0, 1.0, "n.tau", 1)
@@ -85,4 +66,4 @@ class MIQN(_Munchausen, IQN):
                                       self.m_alpha, self.m_tau, self.m_l0, ptr(dtheta), ptr(self._stats), ptr(scratch),
                                       stream_ptr())
         self._backward(dtheta, B)
-        self._finish_step()
+        self._optimizer_step()

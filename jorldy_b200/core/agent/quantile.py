@@ -22,17 +22,12 @@ TAU_STREAM = 0x5141_4E00_0000_0000      # Philox stream id of IQN's fraction dra
 
 
 class _Quantile:
-    """The quantile loss launch and the result dict shared by QRDQN and IQN."""
+    """The quantile loss launch shared by QRDQN and IQN."""
 
     def _quantile_step(self, batch, fwd, tau, tau_stride, layout, N):
         """fwd(net, x, tag) -> quantile output; layout = (sa, sq) of [B, A, K] or [B, N, A]."""
-        B, A = batch["reward"].shape[0], self.action_size
-        state, next_state = self._net_input(batch["state"]), self._net_input(batch["next_state"])
-        reward = batch["reward"].to(torch.float32).reshape(B).contiguous()
-        done = batch["done"].to(torch.float32).reshape(B).contiguous()
-        action = batch["action"].reshape(B).contiguous()
-        if action.dtype not in (torch.int64, torch.int32, torch.float32):
-            action = action.to(torch.int64)
+        B, state, next_state, reward, done, action = self._batch_tensors(batch, 1)
+        A = self.action_size
         net, tgt = self.network, self.target_network
         theta = fwd(net, state, "t.", 0)
         theta_next = fwd(tgt, next_state, "n.", 1)
@@ -45,17 +40,7 @@ class _Quantile:
                            _action_kind(action), ptr(reward), ptr(done), B, A, N, N, self.gamma, ptr(dtheta), ptr(loss),
                            ptr(a_star), ptr(self._stats), ptr(scratch), stream_ptr())
         self._backward(dtheta, B)
-        if self.allreduce is not None:
-            self.allreduce(net.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
-
-    def learn(self):
-        batch, _, _, _ = self._sample()
-        self._learn_batch(batch)
-        st = self._stats[:2].cpu().numpy()
-        self.memory.check_frames()
-        return {"loss": float(st[0]), "epsilon": self.epsilon, "max_Q": float(st[1])}
+        self._optimizer_step()
 
 
 class QRDQN(_Quantile, DQN):

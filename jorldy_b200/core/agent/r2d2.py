@@ -139,10 +139,7 @@ class R2D2(ApeX):
                        self.gamma, float(self.alpha), self.eta, ptr(dq), ptr(prio), ptr(self._stats), ptr(self._scratch),
                        stream_ptr())
         net.backward_tm(tm(dq).view(T * B, A), "t.")
-        if self.allreduce is not None:
-            self.allreduce(net.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
+        self._optimizer_step()
         return prio
 
     def learn(self):

@@ -31,6 +31,8 @@ from .quantile import IQN
 
 
 class RainbowIQN(PER):
+    _decay_eps = False
+
     def __init__(self, state_size, action_size, hidden_size=512, network="rainbow_iqn", head="mlp",
                  optim_config={"name": "adam"}, gamma=0.99, buffer_size=50000, batch_size=64, start_train_step=2000,
                  target_update_period=500, run_step=1e6, lr_decay=True, n_step=4, alpha=0.6, beta=0.4, learn_period=4,
@@ -57,13 +59,15 @@ class RainbowIQN(PER):
 
     _draw_tau = IQN._draw_tau
     process = Rainbow.process
+    learn = Rainbow.learn
     interact_callback = Rainbow.interact_callback
 
     def act_device(self, state, training=True, noise=None):
         """noise: injected draws [(eps_i, eps_j)] x 4 (a1, v1, a2, v2) for this call's single noisy forward."""
         M = state.shape[0]
-        if training and self.memory.size < max(self.batch_size, self.start_train_step):
-            return torch.randint(0, self.action_size, (M,), device=self.device), None
+        action = self._warmup_actions(M, training)
+        if action is not None:
+            return action, None
         A, N = self.action_size, self.num_sample
         tau = self._draw_tau(M, self.sample_min, self.sample_max, "act.tau", 3)
         theta = self.network._buf("act.theta", (M * N, A))
@@ -73,13 +77,8 @@ class RainbowIQN(PER):
         return torch.argmax(q, -1), None
 
     def _learn_batch(self, batch, weights=None):
-        B, A, N = batch["reward"].shape[0], self.action_size, self.num_sample
-        state, next_state = self._net_input(batch["state"]), self._net_input(batch["next_state"])
-        reward = batch["reward"].to(torch.float32).reshape(B, -1).contiguous()
-        done = batch["done"].to(torch.float32).reshape(B, -1).contiguous()
-        action = batch["action"].reshape(B).contiguous()
-        if action.dtype not in (torch.int64, torch.int32, torch.float32):
-            action = action.to(torch.int64)
+        B, state, next_state, reward, done, action = self._batch_tensors(batch)
+        A, N = self.action_size, self.num_sample
         net, tgt = self.network, self.target_network
         noise = self._inject_noise or [None, None, None]
         tau = self._draw_tau(B, 0.0, 1.0, "t.tau", 0)
@@ -97,18 +96,5 @@ class RainbowIQN(PER):
                               float(self.alpha), ptr(dtheta), ptr(loss), ptr(prio), None, ptr(self._stats), ptr(scratch),
                               stream_ptr())
         net.backward(dtheta, tag="t.")
-        if self.allreduce is not None:
-            self.allreduce(net.grad)
-        self.optimizer.step(max_norm=self._clip)
-        self.num_learn += 1
+        self._optimizer_step()
         return prio
-
-    def learn(self):
-        batch, weights, indices, stats_per = self._per_sample()
-        prio = self._learn_batch(batch, weights)
-        self.memory.update_priorities(indices, prio)
-        st = self._stats.cpu().numpy()
-        sp = stats_per.cpu().numpy()
-        self.memory.check_frames()
-        return {"loss": float(st[0]), "beta": self.beta, "max_Q": float(st[1]), "max_logit": float(st[2]),
-                "min_logit": float(st[3]), "sampled_p": float(sp[0]), "mean_p": float(sp[1])}

@@ -32,13 +32,35 @@ def _noisy_init(p, tag, in_f, out_f, noise_type, gen):
     p[f"sig_b{tag}"].fill_(sig_init)
 
 
+def dueling_layers(H, A, K):
+    """The noisy dueling streams' layer table: a1, v1 [H -> H], a2 [H -> A*K], v2 [H -> K] in the reference's call order,
+    on Philox streams 1..4."""
+    return (("_a1", 1, H, H), ("_v1", 2, H, H), ("_a2", 3, H, A * K), ("_v2", 4, H, K))
+
+
 class _NoisyMixin:
+    """A network's noisy layers, listed once in self._noisy as (tag, Philox stream, in, out) in the order the reference
+    calls them.  That table gives their parameter specs (first in state_dict), their init (the generator's last draws)
+    and their noise draws; forward / forward_rows run the network's _body on the effective weights of one draw."""
+
     def _noisy_setup(self, noise_type, seed):
         if noise_type != "factorized":
             raise NotImplementedError("hot-path configs use factorized noise (config/noisy, config/rainbow)")
         self.noise_type = noise_type
         self.noise_seed = int(seed) if seed is not None else 0
         self._draw_ctr = torch.zeros(1, dtype=torch.int64, device=self.device)
+
+    def _noisy_param_specs(self):
+        return [spec for lt, _, i, o in self._noisy for spec in _noisy_specs(lt, i, o)]
+
+    def _noisy_init_params(self, gen):
+        for lt, _, i, o in self._noisy:
+            _noisy_init(self.p, lt, i, o, self.noise_type, gen)
+
+    def _make_noise(self, tag, is_train, noise):
+        """Effective (W, b) of every noisy layer, drawn in table order; noise: injected [(eps_i, eps_j)] per layer."""
+        noise = noise if noise is not None else (None,) * len(self._noisy)
+        return {lt: self._noisy_make(tag, lt, lid, i, o, is_train, nz) for (lt, lid, i, o), nz in zip(self._noisy, noise)}
 
     def _noisy_make(self, tag, lt, layer_id, in_f, out_f, is_train, noise):
         """Draws one layer's factors (or takes injected normals) and returns its effective (W, b), kept under `tag+lt`."""
@@ -63,39 +85,6 @@ class _NoisyMixin:
         if dx is not None:
             L.linear_io_bwd_dx(dy, w, dx, relu_act=relu_act)
 
-
-class Noisy(FlatNetwork, _NoisyMixin):
-    def __init__(self, D_in, D_out, noise_type="factorized", D_hidden=512, head="mlp", device=None, seed=None):
-        super().__init__(device)
-        assert noise_type in ["independent", "factorized"]
-        self._noisy_setup(noise_type, seed)
-        self.D_in, self.D_out, self.D_hidden = D_in, D_out, D_hidden
-        self.head = make_head(head, D_in, D_hidden)
-        F = self.head.D_head_out
-        self._specs = _noisy_specs("1", F, D_hidden) + _noisy_specs("2", D_hidden, D_out) + self.head.specs()
-        self._allocate()
-        self.nout = D_out
-        gen = torch.Generator().manual_seed(seed) if seed is not None else None
-        with torch.no_grad():
-            self.head.init(self.p, gen)
-            _noisy_init(self.p, "1", F, D_hidden, noise_type, gen)
-            _noisy_init(self.p, "2", D_hidden, D_out, noise_type, gen)
-
-    def _make_noise(self, tag, is_train, noise):
-        """Effective (W, b) of the two noisy layers in call order; noise: injected [(eps_i, eps_j)] x 2."""
-        F, H, A = self.head.D_head_out, self.D_hidden, self.D_out
-        n1, n2 = noise if noise is not None else (None, None)
-        return {"1": self._noisy_make(tag, "1", 1, F, H, is_train, n1), "2": self._noisy_make(tag, "2", 2, H, A, is_train, n2)}
-
-    def _body(self, x, idx, M, wb, tag, out, save):
-        feat = self.head.forward(self, x, idx, M, tag, save)
-        h = self._buf(tag + "h", (M, self.D_hidden))
-        L.linear_io_fwd(feat, *wb["1"], h, relu=True)
-        if out is None:
-            out = self._buf(tag + "q", (M, self.D_out))
-        L.linear_io_fwd(h, *wb["2"], out, relu=False)
-        return out
-
     def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
         M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
         return self._body(x, idx, M, self._make_noise(tag, is_train, noise), tag, out, save)
@@ -108,6 +97,62 @@ class Noisy(FlatNetwork, _NoisyMixin):
         for s in range(0, M, self.head.max_rows):
             e = min(M, s + self.head.max_rows)
             self._body(x[s:e], None, e - s, wb, f"inf{e - s}.", out[s:e], False)
+        return out
+
+
+def streams_fwd(net, f, M, A, K, wb, tag, out):
+    """out [M, A, K] = v + a - mean_a a of the noisy dueling streams on f [M, H] (K = 1: one Q per action), with the
+    effective weights wb; the activations stay under `tag` for streams_bwd."""
+    H = net.D_hidden
+    xa = net._buf(tag + "xa", (M, H)); xv = net._buf(tag + "xv", (M, H))
+    L.linear_io_fwd(f, *wb["_a1"], xa, relu=True)
+    L.linear_io_fwd(f, *wb["_v1"], xv, relu=True)
+    a = net._buf(tag + "a", (M, A * K)); v = net._buf(tag + "v", (M, K))
+    L.linear_io_fwd(xa, *wb["_a2"], a, relu=False)
+    L.linear_io_fwd(xv, *wb["_v2"], v, relu=False)
+    C.jb_dueling_fwd(ptr(a), ptr(v), M, A, K, ptr(out), stream_ptr())
+    return out
+
+
+def streams_bwd(net, dout, f, M, A, K, tag):
+    """Writes the four noisy layers' gradients from dout [M, A, K] and returns d loss / d f [M, H] (masked by f > 0)."""
+    H = net.D_hidden
+    xa = net._buf(tag + "xa", (M, H)); xv = net._buf(tag + "xv", (M, H))
+    da = net._buf(tag + "da", (M, A * K)); dv = net._buf(tag + "dv", (M, K))
+    C.jb_dueling_bwd(ptr(dout), M, A, K, ptr(da), ptr(dv), stream_ptr())
+    dxa = net._buf(tag + "dxa", (M, H)); dxv = net._buf(tag + "dxv", (M, H))
+    net._noisy_bwd(da, xa, tag, "_a2", H, A * K, dxa, xa)
+    net._noisy_bwd(dv, xv, tag, "_v2", H, K, dxv, xv)
+    df = net._buf(tag + "df", (M, H)); df2 = net._buf(tag + "df2", (M, H))
+    net._noisy_bwd(dxa, f, tag, "_a1", H, H, df, f)
+    net._noisy_bwd(dxv, f, tag, "_v1", H, H, df2, f)
+    df.add_(df2)
+    return df
+
+
+class Noisy(FlatNetwork, _NoisyMixin):
+    def __init__(self, D_in, D_out, noise_type="factorized", D_hidden=512, head="mlp", device=None, seed=None):
+        super().__init__(device)
+        assert noise_type in ["independent", "factorized"]
+        self._noisy_setup(noise_type, seed)
+        self.D_in, self.D_out, self.D_hidden = D_in, D_out, D_hidden
+        self.head = make_head(head, D_in, D_hidden)
+        self._noisy = (("1", 1, self.head.D_head_out, D_hidden), ("2", 2, D_hidden, D_out))
+        self._specs = self._noisy_param_specs() + self.head.specs()
+        self._allocate()
+        self.nout = D_out
+        gen = torch.Generator().manual_seed(seed) if seed is not None else None
+        with torch.no_grad():
+            self.head.init(self.p, gen)
+            self._noisy_init_params(gen)
+
+    def _body(self, x, idx, M, wb, tag, out, save):
+        feat = self.head.forward(self, x, idx, M, tag, save)
+        h = self._buf(tag + "h", (M, self.D_hidden))
+        L.linear_io_fwd(feat, *wb["1"], h, relu=True)
+        if out is None:
+            out = self._buf(tag + "q", (M, self.D_out))
+        L.linear_io_fwd(h, *wb["2"], out, relu=False)
         return out
 
     def backward(self, dq, M, tag="t."):
@@ -129,72 +174,30 @@ class Rainbow(FlatNetwork, _NoisyMixin):
         self.D_in, self.D_out, self.N_atom, self.D_hidden = D_in, D_out, N_atom, D_hidden
         self.head = make_head(head, D_in, D_hidden)
         F, H = self.head.D_head_out, D_hidden
-        self._specs = (_noisy_specs("_a1", H, H) + _noisy_specs("_v1", H, H) + _noisy_specs("_a2", H, N_atom * D_out)
-                       + _noisy_specs("_v2", H, N_atom) + self.head.specs() + [("l.weight", (H, F)), ("l.bias", (H,))])
+        self._noisy = dueling_layers(H, D_out, N_atom)
+        self._specs = self._noisy_param_specs() + self.head.specs() + [("l.weight", (H, F)), ("l.bias", (H,))]
         self._allocate()
         self.nout = D_out * N_atom
         gen = torch.Generator().manual_seed(seed) if seed is not None else None
         with torch.no_grad():
             self.head.init(self.p, gen)
             self.p["l.weight"].copy_(orthogonal_((H, F), init_gain("relu"), gen))
-            _noisy_init(self.p, "_a1", H, H, noise_type, gen)
-            _noisy_init(self.p, "_v1", H, H, noise_type, gen)
-            _noisy_init(self.p, "_a2", H, N_atom * D_out, noise_type, gen)
-            _noisy_init(self.p, "_v2", H, N_atom, noise_type, gen)
-
-    def _make_noise(self, tag, is_train, noise):
-        """Effective (W, b) of the four noisy layers in the reference's call order a1, v1, a2, v2 (Philox streams 1..4);
-        noise: injected [(eps_i, eps_j)] x 4."""
-        H, AK, K = self.D_hidden, self.D_out * self.N_atom, self.N_atom
-        dims = (("_a1", 1, H, H), ("_v1", 2, H, H), ("_a2", 3, H, AK), ("_v2", 4, H, K))
-        noise = noise if noise is not None else (None,) * 4
-        return {lt: self._noisy_make(tag, lt, lid, i, o, is_train, nz) for (lt, lid, i, o), nz in zip(dims, noise)}
+            self._noisy_init_params(gen)
 
     def _body(self, x, idx, M, wb, tag, out, save):
+        """logits [M, A, K]"""
         H, A, K = self.D_hidden, self.D_out, self.N_atom
         feat = self.head.forward(self, x, idx, M, tag, save)
         f = self._buf(tag + "f", (M, H))
         L.linear_fwd(feat, self.p["l.weight"], self.p["l.bias"], f, relu=True)
-        xa = self._buf(tag + "xa", (M, H)); xv = self._buf(tag + "xv", (M, H))
-        L.linear_io_fwd(f, *wb["_a1"], xa, relu=True)
-        L.linear_io_fwd(f, *wb["_v1"], xv, relu=True)
-        a = self._buf(tag + "a", (M, A * K)); v = self._buf(tag + "v", (M, K))
-        L.linear_io_fwd(xa, *wb["_a2"], a, relu=False)
-        L.linear_io_fwd(xv, *wb["_v2"], v, relu=False)
         if out is None:
             out = self._buf(tag + "logits", (M, A, K))
-        C.jb_dueling_fwd(ptr(a), ptr(v), M, A, K, ptr(out), stream_ptr())
-        return out
-
-    def forward(self, x, is_train=True, idx=None, M=None, out=None, tag="t.", save=True, noise=None):
-        """Returns logits [M, A, K].  noise order = the reference's call order: a1, v1, a2, v2."""
-        M = M if M is not None else (idx.shape[0] if idx is not None else x.shape[0])
-        return self._body(x, idx, M, self._make_noise(tag, is_train, noise), tag, out, save)
-
-    def forward_rows(self, x, out, is_train=True, noise=None):
-        """Chunked inference (act() over many env rows); out [M, A, K].  One noise draw for the whole call, every chunk
-        on the same effective weights (the reference's act() draws once per call).  noise: injected draws (parity tests)."""
-        M = x.shape[0]
-        wb = self._make_noise("inf.", is_train, noise)
-        for s in range(0, M, self.head.max_rows):
-            e = min(M, s + self.head.max_rows)
-            self._body(x[s:e], None, e - s, wb, f"inf{e - s}.", out[s:e], False)
-        return out
+        return streams_fwd(self, f, M, A, K, wb, tag, out)
 
     def backward(self, dlogits, M, tag="t."):
-        H, A, K = self.D_hidden, self.D_out, self.N_atom
         F = self.head.D_head_out
-        feat = self._buf(tag + "head.h", (M, F)); f = self._buf(tag + "f", (M, H))
-        xa = self._buf(tag + "xa", (M, H)); xv = self._buf(tag + "xv", (M, H))
-        da = self._buf(tag + "da", (M, A * K)); dv = self._buf(tag + "dv", (M, K))
-        C.jb_dueling_bwd(ptr(dlogits), M, A, K, ptr(da), ptr(dv), stream_ptr())
-        dxa = self._buf(tag + "dxa", (M, H)); dxv = self._buf(tag + "dxv", (M, H))
-        self._noisy_bwd(da, xa, tag, "_a2", H, A * K, dxa, xa)
-        self._noisy_bwd(dv, xv, tag, "_v2", H, K, dxv, xv)
-        df = self._buf(tag + "df", (M, H)); df2 = self._buf(tag + "df2", (M, H))
-        self._noisy_bwd(dxa, f, tag, "_a1", H, H, df, f)
-        self._noisy_bwd(dxv, f, tag, "_v1", H, H, df2, f)
-        df.add_(df2)
+        feat = self._buf(tag + "head.h", (M, F)); f = self._buf(tag + "f", (M, self.D_hidden))
+        df = streams_bwd(self, dlogits, f, M, self.D_out, self.N_atom, tag)
         L.linear_bwd_dw(df, feat, self.g["l.weight"], self.g["l.bias"])
         dfeat = self._buf(tag + "dfeat", (M, F))
         L.linear_bwd_dx(df, self.p["l.weight"], dfeat, relu_act=feat)

@@ -20,6 +20,7 @@
 // The projection gathers contributions per output atom j in a fixed order over i (no atomics), so
 // results are bit-reproducible.
 #include "common.cuh"
+#include "value_loss.cuh"
 
 namespace {
 
@@ -46,12 +47,6 @@ __device__ __forceinline__ void warp_softmax(const float* __restrict__ x, int K,
   xmax = mx;
   const float m0 = lane < K ? x0 : INFINITY, m1 = lane + 32 < K ? x1 : INFINITY;
   xmin = jb_warp_min(fminf(m0, m1));
-}
-
-__device__ __forceinline__ int read_action(const void* act, int kind, int b) {
-  if (kind == 0) return (int)((const int64_t*)act)[b];
-  if (kind == 1) return ((const int32_t*)act)[b];
-  return (int)((const float*)act)[b];
 }
 
 __global__ void __launch_bounds__(32 * WARPS)
@@ -96,9 +91,7 @@ c51_loss_kernel(const float* __restrict__ logits, const float* __restrict__ next
     for (int h = 0; h < 2; ++h) {
       const int i = lane + 32 * h;
       if (i < K) {
-        float tz = h ? z1 : z0;
-        for (int s = hp.n_step - 1; s >= 0; --s)
-          tz = __fadd_rn(rr[s], __fmul_rn(__fmul_rn(__fadd_rn(1.f, -dr[s]), hp.gamma), tz));
+        const float tz = nstep_fold(h ? z1 : z0, rr, dr, hp.n_step, hp.gamma);
         const float bb = fminf(fmaxf(tz - hp.v_min, 0.f), vrange) / hp.delta_z;
         const float l = floorf(bb), u = ceilf(bb);
         s_l[warp][i] = l; s_u[warp][i] = u; s_wl[warp][i] = u - bb; s_wu[warp][i] = bb - l;
@@ -158,15 +151,6 @@ c51_loss_kernel(const float* __restrict__ logits, const float* __restrict__ next
   }
 }
 
-__global__ void c51_finalize_kernel(const float* __restrict__ partial, int n_cta, int B, float* __restrict__ stats) {
-  if (threadIdx.x != 0) return;
-  float l = 0.f, mq = -INFINITY, ml = -INFINITY, nl = INFINITY;
-  for (int k = 0; k < n_cta; ++k) {
-    l += partial[4 * k]; mq = fmaxf(mq, partial[4 * k + 1]); ml = fmaxf(ml, partial[4 * k + 2]); nl = fminf(nl, partial[4 * k + 3]);
-  }
-  stats[0] = l / (float)B; stats[1] = mq; stats[2] = ml; stats[3] = nl;
-}
-
 }  // namespace
 
 // logits / next_online / next_target: [B, A, K] f32 (next_online may be NULL for variant 0).
@@ -185,7 +169,7 @@ JB_API int jb_c51_loss(const float* logits, const float* next_online, const floa
   cudaStream_t s = (cudaStream_t)stream;
   c51_loss_kernel<<<n_cta, 32 * WARPS, 0, s>>>(logits, next_online, next_target, action, action_kind, reward, done, weights, z,
                                               B, A, K, hp, dlogits, kl, prio, scratch);
-  c51_finalize_kernel<<<1, 32, 0, s>>>(scratch, n_cta, B, stats);
+  loss_logits_finalize_kernel<<<1, 32, 0, s>>>(scratch, n_cta, B, stats);
   return jb_check_launch();
 }
 

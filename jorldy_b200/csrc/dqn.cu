@@ -14,6 +14,7 @@
 #include "common.cuh"
 #include "munchausen.cuh"
 #include "philox.cuh"
+#include "value_loss.cuh"
 
 namespace {
 
@@ -87,12 +88,6 @@ struct TdHP {
   int n_step, double_q, loss_kind /*0 smooth_l1, 1 weighted mse*/, order /*0 dqn, 1 double/per, 2 n-step loop*/;
 };
 
-__device__ __forceinline__ int read_action(const void* act, int kind, int b) {
-  if (kind == 0) return (int)((const int64_t*)act)[b];
-  if (kind == 1) return ((const int32_t*)act)[b];
-  return (int)((const float*)act)[b];
-}
-
 __global__ void __launch_bounds__(1024)
 td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, const float* __restrict__ qt_next,
                const void* __restrict__ action, int action_kind, const float* __restrict__ reward,
@@ -100,7 +95,7 @@ td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, co
                float* __restrict__ dq, double* __restrict__ prio, float* __restrict__ stats) {
   __shared__ float s_loss[32], s_max[32];
   const int b = threadIdx.x;
-  float loss_b = 0.f, q_b = -INFINITY;
+  float q_b = -INFINITY, loss_b = 0.f;
   if (b < B) {
     const int a = read_action(action, action_kind, b);
     const float* qr = q + (size_t)b * A;
@@ -109,10 +104,7 @@ td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, co
     // bootstrap value
     float y;
     if (hp.double_q) {
-      const float* nr = q_next + (size_t)b * A;
-      int am = 0; float best = nr[0];
-      for (int i = 1; i < A; ++i) if (nr[i] > best) { best = nr[i]; am = i; }
-      y = tr[am];
+      y = tr[first_argmax(q_next + (size_t)b * A, A)];
     } else {
       y = tr[0];
       for (int i = 1; i < A; ++i) y = fmaxf(y, tr[i]);
@@ -121,10 +113,7 @@ td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, co
     const float* dr = done + (size_t)b * hp.n_step;
     if (hp.order == 0)       y = __fadd_rn(rr[0], __fmul_rn(__fmul_rn(__fadd_rn(1.f, -dr[0]), hp.gamma), y));
     else if (hp.order == 1)  y = __fadd_rn(rr[0], __fmul_rn(y, __fmul_rn(hp.gamma, __fadd_rn(1.f, -dr[0]))));
-    else {
-      for (int i = hp.n_step - 1; i >= 0; --i)
-        y = __fadd_rn(rr[i], __fmul_rn(__fmul_rn(__fadd_rn(1.f, -dr[i]), hp.gamma), y));
-    }
+    else                     y = nstep_fold(y, rr, dr, hp.n_step, hp.gamma);
     const float diff = q_b - y;
     float g;
     if (hp.loss_kind == 0) {                    // F.smooth_l1_loss(q, y), beta = 1, mean
@@ -156,7 +145,7 @@ td_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, co
 
 // ---- Munchausen DQN loss (arXiv:2007.14430) ------------------------------------------------------
 // One warp per sample; lane 0 forms the target in a fixed order (munchausen.cuh), the warp writes the sample's dq row.
-// The per-sample loss and Q(s)[a_t] go to partial[2b], partial[2b + 1] and one thread folds them (mdqn_finalize_kernel).
+// The per-sample loss and Q(s)[a_t] go to partial[2b], partial[2b + 1] and one thread folds them (loss_maxq_finalize_kernel).
 constexpr int MDQN_WARPS = 4;
 
 __global__ void __launch_bounds__(MDQN_WARPS * 32)
@@ -185,14 +174,6 @@ mdqn_loss_kernel(const float* __restrict__ q, const float* __restrict__ qt_s, co
   }
   g = __shfl_sync(0xffffffffu, g, 0) / (float)B;
   for (int a = lane; a < A; a += 32) dq[(size_t)b * A + a] = a == a_t ? g : 0.f;
-}
-
-__global__ void mdqn_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
-  if (threadIdx.x != 0) return;
-  float l = 0.f, mq = -INFINITY;
-  for (int b = 0; b < B; ++b) { l += partial[2 * b]; mq = fmaxf(mq, partial[2 * b + 1]); }
-  stats[0] = l / (float)B;   // loss
-  stats[1] = mq;             // max_Q = max over the batch of Q(s)[a], as td_loss_kernel
 }
 
 }  // namespace
@@ -245,6 +226,6 @@ JB_API int jb_mdqn_loss(const float* q, const float* qt_s, const float* qt_next,
   cudaStream_t s = (cudaStream_t)stream;
   mdqn_loss_kernel<<<jb_div_up(B, MDQN_WARPS), MDQN_WARPS * 32, 0, s>>>(q, qt_s, qt_next, action, action_kind, reward, done,
                                                                        B, A, gamma, m_alpha, m_tau, l0, dq, scratch);
-  mdqn_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  loss_maxq_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }

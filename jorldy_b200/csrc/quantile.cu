@@ -14,6 +14,7 @@
 #include "common.cuh"
 #include "munchausen.cuh"
 #include "philox.cuh"
+#include "value_loss.cuh"
 
 namespace {
 
@@ -21,12 +22,6 @@ constexpr int QMAXN = 256;     // quantiles per pass (N, N')
 constexpr int QMAXA = 18;      // ALE's full action set
 constexpr int QT = 256;        // threads per CTA of the loss kernel: one predicted quantile each
 static_assert(QMAXA == MUNCHAUSEN_MAX_A, "M-IQN's pi' / tau logpi' rows hold every action");
-
-__device__ __forceinline__ int read_action(const void* act, int kind, int b) {
-  if (kind == 0) return (int)((const int64_t*)act)[b];
-  if (kind == 1) return ((const int32_t*)act)[b];
-  return (int)((const float*)act)[b];
-}
 
 // mean of x[0], x[sq], ..., x[(n-1) sq] over one warp: lane-strided partial sums, then the butterfly.  The loss kernel
 // and jb_quantile_mean share it, so a* / max_Q and act()'s greedy action come from bit-identical means.
@@ -178,17 +173,10 @@ rainbow_iqn_loss_kernel(const float* __restrict__ pred, const float* __restrict_
   if (lane == 0) { s_mx[warp] = mx; s_mn[warp] = mn; }
   for (int i = tid; i < N; i += QT) s_tau[i] = tau[(size_t)b * N + i];
   __syncthreads();
-  int a_star = 0;
-  float best = s_qn[0];
-  for (int a = 1; a < A; ++a)
-    if (s_qn[a] > best) { best = s_qn[a]; a_star = a; }
+  const int a_star = first_argmax(s_qn, A);
   const float* rr = reward + (size_t)b * n_step;
   const float* dr = done + (size_t)b * n_step;
-  for (int j = tid; j < Np; j += QT) {
-    float y = tb[(size_t)j * A + a_star];
-    for (int s = n_step - 1; s >= 0; --s) y = __fadd_rn(rr[s], __fmul_rn(__fmul_rn(__fadd_rn(1.f, -dr[s]), gamma), y));
-    s_y[j] = y;
-  }
+  for (int j = tid; j < Np; j += QT) s_y[j] = nstep_fold(tb[(size_t)j * A + a_star], rr, dr, n_step, gamma);
   const int a_t = read_action(action, action_kind, b);
   const double w = weights ? weights[b] : 1.0;
   const float gcoef = (float)(w / ((double)B * (double)Np));
@@ -206,24 +194,6 @@ rainbow_iqn_loss_kernel(const float* __restrict__ pred, const float* __restrict_
     partial[4 * b + 2] = mx;
     partial[4 * b + 3] = mn;
   }
-}
-
-__global__ void rainbow_iqn_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
-  if (threadIdx.x != 0) return;
-  float l = 0.f, mq = -INFINITY, ml = -INFINITY, nl = INFINITY;
-  for (int b = 0; b < B; ++b) {
-    l += partial[4 * b];
-    mq = fmaxf(mq, partial[4 * b + 1]); ml = fmaxf(ml, partial[4 * b + 2]); nl = fminf(nl, partial[4 * b + 3]);
-  }
-  stats[0] = l / (float)B; stats[1] = mq; stats[2] = ml; stats[3] = nl;
-}
-
-__global__ void quantile_finalize_kernel(const float* __restrict__ partial, int B, float* __restrict__ stats) {
-  if (threadIdx.x != 0) return;
-  float l = 0.f, mq = -INFINITY;
-  for (int b = 0; b < B; ++b) { l += partial[2 * b]; mq = fmaxf(mq, partial[2 * b + 1]); }
-  stats[0] = l / (float)B;
-  stats[1] = mq;
 }
 
 __global__ void quantile_mean_kernel(const float* __restrict__ x, int sa, int sq, int M, int A, int N, float* __restrict__ q) {
@@ -251,7 +221,7 @@ JB_API int jb_quantile_loss(const float* pred, int p_sa, int p_sq, const float* 
   cudaStream_t s = (cudaStream_t)stream;
   quantile_loss_kernel<<<B, QT, 0, s>>>(pred, p_sa, p_sq, next_target, t_sa, t_sq, tau, tau_stride, action, action_kind,
                                         reward, done, A, N, Np, gamma, gcoef, dpred, loss, a_star, scratch);
-  quantile_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  loss_maxq_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }
 
@@ -269,7 +239,7 @@ JB_API int jb_munchausen_quantile_loss(const float* pred, const float* next_targ
   munchausen_quantile_loss_kernel<<<B, QT, 0, s>>>(pred, next_target, cur_target, tau, tau_stride, action, action_kind,
                                                    reward, done, A, N, Np, Nc, gamma, m_alpha, m_tau, l0, gcoef, dpred,
                                                    scratch);
-  quantile_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  loss_maxq_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
   return jb_check_launch();
 }
 
@@ -286,7 +256,7 @@ JB_API int jb_rainbow_iqn_loss(const float* pred, const float* next_online, cons
   cudaStream_t s = (cudaStream_t)stream;
   rainbow_iqn_loss_kernel<<<B, QT, 0, s>>>(pred, next_online, next_target, tau, action, action_kind, reward, done, weights, B,
                                            A, N, Nn, Np, n_step, gamma, alpha, dpred, loss, prio, a_star, scratch);
-  rainbow_iqn_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, stats);
+  loss_logits_finalize_kernel<<<1, 32, 0, s>>>(scratch, B, B, stats);
   return jb_check_launch();
 }
 

@@ -7,6 +7,7 @@
 // sequences in order in the single-thread finalize): bit-reproducible, no atomics.  The target of a step is formed in
 // float64 (h^-1 of a value near 0 cancels in its last step), the loss partials too; dq is rounded once to fp32.
 #include "common.cuh"
+#include "value_loss.cuh"
 
 namespace {
 
@@ -37,12 +38,7 @@ r2d2_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next, 
   float mq = -INFINITY;
   for (int t = tid; t < T; t += RT) {
     const size_t row = ((size_t)b * T + t) * A;
-    const float* qn = q_next + row;
-    int a_star = 0;
-    float best = qn[0];
-    for (int a = 1; a < A; ++a)
-      if (qn[a] > best) { best = qn[a]; a_star = a; }      // first index on ties, like torch.argmax
-    double y = value_h_inv((double)qt_next[row + a_star]);
+    double y = value_h_inv((double)qt_next[row + first_argmax(q_next + row, A)]);
     for (int i = n - 1; i >= 0; --i) y = (double)rr[t + i] + (1.0 - (double)dr[t + i]) * (double)gamma * y;
     y = value_h(y);
     const int a_t = (int)action[(size_t)b * T + t];
