@@ -9,6 +9,21 @@ import torch
 from ..dev import f32
 
 
+def cpu_state_dict(net):
+    """A network's state_dict with every tensor copied to the CPU, as checkpoints store it."""
+    return {k: v.cpu() for k, v in net.state_dict().items()}
+
+
+def cpu_optimizer_state(optimizer):
+    """An optimizer's state_dict with every state tensor copied to the CPU, as checkpoints store it."""
+    sd = optimizer.state_dict()
+    for st in sd["state"].values():
+        for k, v in st.items():
+            if torch.is_tensor(v):
+                st[k] = v.cpu()
+    return sd
+
+
 class BaseAgent(ABC):
     @abstractmethod
     def act(self, state):
@@ -21,6 +36,23 @@ class BaseAgent(ABC):
     @abstractmethod
     def process(self, transitions, step):
         ...
+
+    def _state_to_device(self, state):
+        """act()'s input as a tensor: a tensor is used as it is, anything else is copied to the agent's device."""
+        return state if isinstance(state, torch.Tensor) else torch.as_tensor(np.asarray(state), device=self.device)
+
+    def _row_counter(self, M):
+        """Device int64 [M] per-row Philox draw counters of the act kernels for batches of M rows, created on first use.
+        The kernels read and advance them on the device, so CUDA-graph replays draw fresh numbers."""
+        ctr = self._row_ctr.get(M)
+        if ctr is None:
+            ctr = self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        return ctr
+
+    def _replay_indices(self, device=None):
+        """int64 replay indices of the next learn(): the injected ones if a test set them, else a uniform sample."""
+        src = self._inject_idx if self._inject_idx is not None else self.memory.sample_indices(self.batch_size)
+        return torch.as_tensor(np.asarray(src), dtype=torch.int64, device=device)
 
     def as_tensor(self, x):
         if isinstance(x, list):
@@ -64,13 +96,8 @@ class BaseAgent(ABC):
     # checkpoint format = the reference's: {"network": state_dict, "optimizer": state_dict} -> path/ckpt
     def save(self, path):
         print(f"...Save model to {path}...")
-        net = {k: v.cpu() for k, v in self.network.state_dict().items()}
-        opt = self.optimizer.state_dict()
-        for st in opt["state"].values():
-            for k, v in st.items():
-                if torch.is_tensor(v):
-                    st[k] = v.cpu()
-        torch.save({"network": net, "optimizer": opt}, os.path.join(path, "ckpt"))
+        torch.save({"network": cpu_state_dict(self.network), "optimizer": cpu_optimizer_state(self.optimizer)},
+                   os.path.join(path, "ckpt"))
 
     def load(self, path):
         print(f"...Load model from {path}...")

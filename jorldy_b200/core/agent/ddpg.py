@@ -18,7 +18,7 @@ from ..dev import C, ptr, require_cuda, stream_ptr
 from ..network import Network
 from ..network.base import FlatNetwork
 from ..optimizer import Optimizer
-from .base import BaseAgent
+from .base import BaseAgent, cpu_optimizer_state, cpu_state_dict
 
 _DEFAULT_OPTIM = {"actor": "adam", "critic": "adam", "actor_lr": 5e-4, "critic_lr": 1e-3}
 
@@ -36,6 +36,8 @@ class _Scalar(FlatNetwork):
 class _ActorCritic(BaseAgent):
     action_type = "continuous"
     _n_critics = 1
+    _strict_gate = False        # learn once memory.size > batch_size (SAC) instead of >= batch_size (DDPG, TD3)
+    _soft_in_process = True     # process() soft-updates the targets (TD3 does it inside its delayed learn() steps)
 
     def _common(self, state_size, action_size, hidden_size, actor, critic, head, optim_config, gamma, buffer_size, batch_size,
                 start_train_step, tau, run_step, lr_decay, device, seed, target_actor, use_cuda_graph=True):
@@ -88,15 +90,8 @@ class _ActorCritic(BaseAgent):
     def _net_input(self, s):
         return s.to(torch.float32).reshape(s.shape[0], -1)
 
-    def _state_to_device(self, state):
-        return state if isinstance(state, torch.Tensor) else torch.as_tensor(np.asarray(state), device=self.device)
-
     def _sample(self):
-        if self._inject_idx is not None:
-            idx = torch.as_tensor(np.asarray(self._inject_idx), dtype=torch.int64, device=self.device)
-        else:
-            idx = torch.as_tensor(self.memory.sample_indices(self.batch_size), dtype=torch.int64, device=self.device)
-        return self.memory.gather_device(idx)
+        return self.memory.gather_device(self._replay_indices(self.device))
 
     def _unpack(self, batch):
         B = batch["reward"].shape[0]
@@ -146,8 +141,7 @@ class _ActorCritic(BaseAgent):
         B = self.batch_size
         if self._idx_buf is None:
             self._idx_buf = torch.zeros(B, dtype=torch.int64, device=self.device)
-        src = self._inject_idx if self._inject_idx is not None else self.memory.sample_indices(B)
-        self._idx_buf.copy_(torch.as_tensor(np.asarray(src), dtype=torch.int64))
+        self._idx_buf.copy_(self._replay_indices())
         for opt in self._all_optimizers():
             opt._sync_lr()                       # graph replays do not pass through optimizer.step()'s host-side lr check
         key = self._variant()
@@ -164,25 +158,30 @@ class _ActorCritic(BaseAgent):
             g.replay()
         return self._finish()
 
-    # ---- checkpoints: the reference's key layout (ddpg.py:176-197, td3.py:222-246, sac.py:306-339) ---------------------
-    @staticmethod
-    def _cpu_opt(opt):
-        sd = opt.state_dict()
-        for st in sd["state"].values():
-            for k, v in st.items():
-                if torch.is_tensor(v):
-                    st[k] = v.cpu()
-        return sd
+    def process(self, transitions, step):
+        """ddpg.py / td3.py / sac.py process(): store; learn and decay the learning rates once the replay holds a batch and
+        step >= start_train_step; then, once learning has started, soft-update the targets on every call."""
+        result = {}
+        self.memory.store(transitions)
+        filled = self.memory.size > self.batch_size if self._strict_gate else self.memory.size >= self.batch_size
+        if filled and step >= self.start_train_step:
+            result = self.learn()
+            if self.lr_decay:
+                self.learning_rate_decay(step, self._optimizers())
+        if self._soft_in_process and self.num_learn > 0:
+            self.update_target_soft()
+        return result
 
+    # ---- checkpoints: the reference's key layout (ddpg.py:176-197, td3.py:222-246, sac.py:306-339) ---------------------
     def _ckpt(self):
-        d = {"actor": {k: v.cpu() for k, v in self.actor.state_dict().items()}, "actor_optimizer": self._cpu_opt(self.actor_optimizer)}
+        d = {"actor": cpu_state_dict(self.actor), "actor_optimizer": cpu_optimizer_state(self.actor_optimizer)}
         if self._n_critics == 1:
-            d["critic"] = {k: v.cpu() for k, v in self.critics[0].state_dict().items()}
-            d["critic_optimizer"] = self._cpu_opt(self.critic_optimizers[0])
+            d["critic"] = cpu_state_dict(self.critics[0])
+            d["critic_optimizer"] = cpu_optimizer_state(self.critic_optimizers[0])
         else:
             for i in (0, 1):
-                d[f"critic{i + 1}"] = {k: v.cpu() for k, v in self.critics[i].state_dict().items()}
-                d[f"critic_optimizer{i + 1}"] = self._cpu_opt(self.critic_optimizers[i])
+                d[f"critic{i + 1}"] = cpu_state_dict(self.critics[i])
+                d[f"critic_optimizer{i + 1}"] = cpu_optimizer_state(self.critic_optimizers[i])
         return d
 
     def save(self, path):
@@ -231,9 +230,9 @@ class DDPG(_ActorCritic):
         self.actor.forward_rows(state, pre)
         if M not in self._ou:
             self._ou[M] = torch.full((M, A), self.ou_mu, dtype=torch.float64, device=self.device)
-            self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        row_ctr = self._row_counter(M)
         action = self.actor._buf("act.a", (M, A))
-        C.jb_ou_act(ptr(pre), M, A, ptr(self._ou[M]), ptr(noise), self.seed, self.rng_stream_base, ptr(self._row_ctr[M]),
+        C.jb_ou_act(ptr(pre), M, A, ptr(self._ou[M]), ptr(noise), self.seed, self.rng_stream_base, ptr(row_ctr),
                     self.ou_theta, self.ou_mu, self.ou_sigma, 0 if training else 1, ptr(action), stream_ptr())
         return action, None
 
@@ -267,21 +266,11 @@ class DDPG(_ActorCritic):
         self.actor.backward_raw(dpre, B, tag="t.")
         self.actor_optimizer.step()
 
-    def process(self, transitions, step):
-        result = {}
-        self.memory.store(transitions)
-        if self.memory.size >= self.batch_size and step >= self.start_train_step:
-            result = self.learn()
-            if self.lr_decay:
-                self.learning_rate_decay(step, self._optimizers())
-        if self.num_learn > 0:
-            self.update_target_soft()
-        return result
-
 
 class TD3(DDPG):
     """jorldy/core/agent/td3.py:13-265: twin critics, clipped target-policy smoothing, delayed actor + target updates."""
     _n_critics = 2
+    _soft_in_process = False
 
     def __init__(self, state_size, action_size, hidden_size=512, actor="deterministic_policy", critic="continuous_q_network",
                  head="mlp", optim_config=_DEFAULT_OPTIM, gamma=0.99, buffer_size=50000, batch_size=128,
@@ -345,21 +334,13 @@ class TD3(DDPG):
             self.actor_loss = float(st[4])
         return {"critic_loss1": float(st[0]), "critic_loss2": float(st[1]), "actor_loss": self.actor_loss, "max_Q": float(st[2])}
 
-    def process(self, transitions, step):
-        result = {}
-        self.memory.store(transitions)
-        if self.memory.size >= self.batch_size and step >= self.start_train_step:
-            result = self.learn()
-            if self.lr_decay:
-                self.learning_rate_decay(step, self._optimizers())
-        return result
-
 
 class SAC(_ActorCritic):
     """jorldy/core/agent/sac.py:16-355, continuous actions (`actor="continuous_policy"`); `actor="discrete_policy"`
     constructs the discrete-action SAC (SACDiscrete below)."""
     _n_critics = 2
     _actor_kind = "continuous"
+    _strict_gate = True
 
     def __new__(cls, *args, **kwargs):
         actor = kwargs.get("actor", args[3] if len(args) > 3 else "continuous_policy")
@@ -371,6 +352,7 @@ class SAC(_ActorCritic):
                  head="mlp", optim_config=dict(_DEFAULT_OPTIM, alpha="adam", alpha_lr=3e-4), use_dynamic_alpha=False,
                  gamma=0.99, tau=5e-3, buffer_size=50000, batch_size=64, start_train_step=2000, static_log_alpha=-2.0,
                  target_update_period=10000, run_step=1e6, lr_decay=True, device=None, seed=0, use_cuda_graph=True, **kwargs):
+        # target_update_period is accepted because the reference's configs pass it; the targets follow the soft update
         if actor.split("_")[0] != self._actor_kind:
             raise NotImplementedError(f"actor '{actor}': SAC is built with continuous_policy and discrete_policy actors")
         self._common(state_size, action_size, hidden_size, actor, critic, head, optim_config, gamma, buffer_size, batch_size,
@@ -381,17 +363,15 @@ class SAC(_ActorCritic):
                                 if use_dynamic_alpha else None)
         self.alpha = self.log_alpha.flat[:1].exp()       # device scalar; refreshed inside learn() like sac.py:241
         self.target_entropy = -float(action_size)
-        self.target_update_stamp, self.time_t, self.target_update_period = 0, 0, target_update_period
 
     def act_device(self, state, training=True, noise=None):
         """sac.py:139-142: a = tanh(Normal(mu, std).sample()) when training, tanh(mu) otherwise."""
         M, A = state.shape[0], self.action_size
         raw = self.actor._buf("act.raw", (M, 2 * A))
         self.actor.forward_rows(state, raw)
-        if M not in self._row_ctr:
-            self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        row_ctr = self._row_counter(M)
         action = self.actor._buf("act.a", (M, A))
-        C.jb_ppo_act_continuous(ptr(raw), M, A, 2 * A, ptr(noise), self.seed, self.rng_stream_base, 0, ptr(self._row_ctr[M]),
+        C.jb_ppo_act_continuous(ptr(raw), M, A, 2 * A, ptr(noise), self.seed, self.rng_stream_base, 0, ptr(row_ctr),
                                 0 if training else 1, ptr(action), stream_ptr())
         return action, None
 
@@ -445,25 +425,11 @@ class SAC(_ActorCritic):
         return {"critic_loss1": float(h[0]), "critic_loss2": float(h[1]), "actor_loss": float(h[4]), "alpha_loss": float(h[8]),
                 "max_Q": float(h[2]), "mean_Q": float(h[5]), "alpha": float(h[9]), "entropy": float(h[6])}
 
-    def process(self, transitions, step):
-        result = {}
-        self.memory.store(transitions)
-        delta_t = step - self.time_t
-        self.time_t = step
-        self.target_update_stamp += delta_t
-        if self.memory.size > self.batch_size and step >= self.start_train_step:
-            result = self.learn()
-            if self.lr_decay:
-                self.learning_rate_decay(step, self._optimizers())
-        if self.num_learn > 0:
-            self.update_target_soft()
-        return result
-
     def _ckpt(self):
         d = super()._ckpt()
         if self.use_dynamic_alpha:
             d["log_alpha"] = self.log_alpha.flat[:1].detach().cpu().clone()
-            d["alpha_optimizer"] = self._cpu_opt(self.alpha_optimizer)
+            d["alpha_optimizer"] = cpu_optimizer_state(self.alpha_optimizer)
         return d
 
     def load(self, path):
@@ -512,10 +478,9 @@ class SACDiscrete(SAC):
         M, A = state.shape[0], self.action_size
         logits = self.actor._buf("act.z", (M, A))
         self.actor.forward_rows(state, logits)
-        if M not in self._row_ctr:
-            self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        row_ctr = self._row_counter(M)
         action = self.actor._buf("act.a", (M, 1), torch.int64)
-        C.jb_sacd_act(ptr(logits), M, A, ptr(noise), self.seed, self.rng_stream_base, ptr(self._row_ctr[M]),
+        C.jb_sacd_act(ptr(logits), M, A, ptr(noise), self.seed, self.rng_stream_base, ptr(row_ctr),
                       0 if training else 1, ptr(action), stream_ptr())
         return action, None
 

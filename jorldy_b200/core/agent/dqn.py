@@ -93,21 +93,12 @@ class DQN(BaseAgent):
         M = state.shape[0]
         q = self._q_values(state, training)
         eps = self.epsilon if training else self.epsilon_eval
-        row_ctr = self._row_ctr.get(M)
-        if row_ctr is None:
-            row_ctr = self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
         action = self.network._buf("act.a", (M,), torch.int64)
         q_sel = self.network._buf("act.qsel", (M,))
         eps_rows = self._eps_rows if (training and self._eps_rows is not None and self._eps_rows.shape[0] == M) else None
         C.jb_q_act(ptr(q), M, self.action_size, float(eps), ptr(eps_rows), ptr(noise), self.seed, self.rng_stream_base,
-                   ptr(row_ctr), ptr(action), ptr(q_sel), stream_ptr())
+                   ptr(self._row_counter(M)), ptr(action), ptr(q_sel), stream_ptr())
         return action, q_sel
-
-    def _state_to_device(self, state):
-        if isinstance(state, torch.Tensor):
-            return state
-        a = np.asarray(state)
-        return torch.as_tensor(a, device=self.device)
 
     def _net_input(self, s):
         """uint8 frames stay uint8 for the CNN head (it scales by 1/255 itself); vectors -> f32 [N, D]."""
@@ -125,12 +116,7 @@ class DQN(BaseAgent):
     # ------------------------------------------------------------------------------------ learn --
     def _sample(self):
         """Returns (batch dict of device tensors, weights f64|None, tree indices|None, stats|None)."""
-        idx = None
-        if self._inject_idx is not None:
-            idx = torch.as_tensor(np.asarray(self._inject_idx), dtype=torch.int64, device=self.device)
-        else:
-            idx = torch.as_tensor(self.memory.sample_indices(self.batch_size), dtype=torch.int64, device=self.device)
-        return self.memory.gather_device(idx), None, None, None
+        return self.memory.gather_device(self._replay_indices(self.device)), None, None, None
 
     def _forward_q(self, net, x, tag, is_train=True, noise=None):
         return net.forward(x, tag=tag)

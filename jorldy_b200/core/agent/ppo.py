@@ -110,9 +110,7 @@ class PPO(BaseAgent):
         out = net._buf("act.out", (M, net.nout))
         net.forward_rows(state, out)
         A = self.action_size
-        row_ctr = self._row_ctr.get(M)
-        if row_ctr is None:
-            row_ctr = self._row_ctr[M] = torch.zeros(M, dtype=torch.int64, device=self.device)
+        row_ctr = self._row_counter(M)
         if self.continuous:
             action = net._buf("act.a", (M, A))
             C.jb_ppo_act_continuous(ptr(out), M, A, net.nout, ptr(noise), self.seed, self.rng_stream_base,

@@ -10,16 +10,6 @@ namespace {
 
 constexpr int AC_MAX_A = 8;
 
-// Box-Muller pair from one Philox draw (same construction as ppo_act_continuous_kernel, ppo.cu).
-__device__ __forceinline__ void normal_pair(uint64_t seed, uint64_t stream, uint64_t ctr, float& n0, float& n1) {
-  jb_philox4 r = jb_philox(seed, stream, ctr);
-  const float u1 = (float)((r.x >> 8) + 1u) * (1.0f / 16777216.0f);   // (0,1]
-  const float u2 = jb_u01_float(r.y);
-  const float rad = sqrtf(-2.0f * logf(u1));
-  n0 = rad * cospif(2.0f * u2);
-  n1 = rad * sinpif(2.0f * u2);
-}
-
 // ---- t := tau * p + (1 - tau) * t  (ddpg.py:160-164, td3.py:190-196, sac.py:262-266) ---------------------------------
 // torch evaluates `tau * p.data + (1 - tau) * t_p.data` as two rounded products and one rounded sum: no FMA here.
 __global__ void soft_update_kernel(float* __restrict__ t, const float* __restrict__ p, long long n, float tau, float omt) {
@@ -69,10 +59,9 @@ __global__ void ou_act_kernel(const float* __restrict__ pre, int M, int A, doubl
   if (!greedy) {
     if (n_in) nz = n_in[m];
     else {
-      uint64_t ctr = 0;
-      if (row_ctr) { ctr = (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
+      const uint64_t ctr = jb_next_row_ctr(row_ctr, m);
       float n0, n1;
-      normal_pair(seed, stream_base + (uint64_t)m, ctr, n0, n1);
+      jb_normal_pair(seed, stream_base + (uint64_t)m, ctr, n0, n1);
       nz = (double)n0;
     }
   }
@@ -93,7 +82,7 @@ __global__ void philox_fill_kernel(float* __restrict__ out, long long n, int kin
   if (2 * p >= n) return;
   if (ctr_dev) ctr += (uint64_t)ctr_dev[0];
   float v0, v1;
-  if (kind == 0) normal_pair(seed, stream + (uint64_t)p, ctr, v0, v1);
+  if (kind == 0) jb_normal_pair(seed, stream + (uint64_t)p, ctr, v0, v1);
   else {
     jb_philox4 r = jb_philox(seed, stream + (uint64_t)p, ctr);
     v0 = lo + (hi - lo) * jb_u01_float(r.x);
@@ -302,11 +291,7 @@ __global__ void sacd_act_kernel(const float* __restrict__ z, int M, int A, const
   } else {
     float u;
     if (u_in) u = u_in[m];
-    else {
-      uint64_t ctr = 0;
-      if (row_ctr) { ctr = (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
-      u = jb_u01_float(jb_philox(seed, stream_base + (uint64_t)m, ctr).x);
-    }
+    else u = jb_u01_float(jb_philox(seed, stream_base + (uint64_t)m, jb_next_row_ctr(row_ctr, m)).x);
     float tot = 0.f;
 #pragma unroll
     for (int a = 0; a < SACD_MAX_A; ++a) if (a < A) tot += expf(lp[a]);

@@ -32,8 +32,7 @@ __global__ void q_act_kernel(const float* __restrict__ q, int M, int A, float ep
   float u0, u1;
   if (u_in) { u0 = u_in[2 * m]; u1 = u_in[2 * m + 1]; }
   else {
-    uint64_t c = 0;
-    if (row_ctr) { c = (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
+    const uint64_t c = jb_next_row_ctr(row_ctr, m);
     jb_philox4 r = jb_philox(seed, stream_base + (uint64_t)m, c);
     u0 = jb_u01_float(r.x); u1 = jb_u01_float(r.y);
   }

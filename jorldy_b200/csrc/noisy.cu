@@ -35,10 +35,9 @@ __global__ void noisy_factors_kernel(const float* __restrict__ eps_i, const floa
   if (inj) e = (t < in_f) ? eps_i[t] : eps_j[t - in_f];
   else {
     const uint64_t c = ctr_ptr ? (uint64_t)(*ctr_ptr) : 0;
-    jb_philox4 r = jb_philox(seed, stream, c * DRAW_STRIDE + (uint64_t)(t >> 1));
-    const float u1 = (float)((r.x >> 8) + 1u) * (1.0f / 16777216.0f), u2 = jb_u01_float(r.y);
-    const float rad = sqrtf(-2.0f * logf(u1));
-    e = (t & 1) ? rad * sinpif(2.0f * u2) : rad * cospif(2.0f * u2);
+    float n0, n1;
+    jb_normal_pair(seed, stream, c * DRAW_STRIDE + (uint64_t)(t >> 1), n0, n1);
+    e = (t & 1) ? n1 : n0;
   }
   const float f = f_noise(e);
   if (t < in_f) f_i[t] = f; else f_j[t - in_f] = f;

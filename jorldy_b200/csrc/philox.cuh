@@ -50,3 +50,20 @@ __host__ __device__ __forceinline__ double jb_u01_double(uint32_t a, uint32_t b)
 __host__ __device__ __forceinline__ float jb_u01_float(uint32_t a) {
   return (float)(a >> 8) * (1.0f / 16777216.0f);
 }
+
+// Two standard normals from one Philox draw by Box-Muller: u1 in (0,1] from x (so logf stays finite), u2 in [0,1) from y.
+__device__ __forceinline__ void jb_normal_pair(uint64_t seed, uint64_t stream, uint64_t ctr, float& n0, float& n1) {
+  jb_philox4 r = jb_philox(seed, stream, ctr);
+  const float u1 = (float)((r.x >> 8) + 1u) * (1.0f / 16777216.0f);
+  const float u2 = jb_u01_float(r.y);
+  const float rad = sqrtf(-2.0f * logf(u1));
+  n0 = rad * cospif(2.0f * u2);
+  n1 = rad * sinpif(2.0f * u2);
+}
+
+// Per-row draw counter of the act kernels: returns base + row_ctr[m] and advances row_ctr[m], so that every launch (and
+// every CUDA-graph replay) draws fresh numbers; base when there is no counter.
+__device__ __forceinline__ uint64_t jb_next_row_ctr(long long* __restrict__ row_ctr, int m, uint64_t base = 0) {
+  if (row_ctr) { base += (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
+  return base;
+}

@@ -40,7 +40,7 @@ __global__ void ppo_act_discrete_kernel(const float* __restrict__ out, int M, in
                                         int64_t* __restrict__ action) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
-  if (row_ctr) { ctr += (uint64_t)row_ctr[m]; row_ctr[m] += 1; }   // per-row draw counter (graph-replay safe)
+  ctr = jb_next_row_ctr(row_ctr, m, ctr);
   float lg[NA], lsm[NA];
 #pragma unroll
   for (int a = 0; a < NA; ++a) lg[a] = a < A ? out[(size_t)m * nout + a] : 0.f;
@@ -74,19 +74,12 @@ __global__ void ppo_act_continuous_kernel(const float* __restrict__ out, int M, 
                                           float* __restrict__ action) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
-  if (row_ctr) { ctr += (uint64_t)row_ctr[m]; row_ctr[m] += 1; }
+  ctr = jb_next_row_ctr(row_ctr, m, ctr);
   for (int a = 0; a < A; a += 2) {
     float n0 = 0.f, n1 = 0.f;
     if (!greedy) {
       if (n_in) { n0 = n_in[(size_t)m * A + a]; if (a + 1 < A) n1 = n_in[(size_t)m * A + a + 1]; }
-      else {
-        // Box-Muller on two Philox uniforms
-        jb_philox4 r = jb_philox(seed, stream_base + (uint64_t)m, ctr * 8 + (uint64_t)(a >> 1));
-        const float u1 = (float)((r.x >> 8) + 1u) * (1.0f / 16777216.0f);   // (0,1]
-        const float u2 = jb_u01_float(r.y);
-        const float rad = sqrtf(-2.0f * logf(u1));
-        n0 = rad * cospif(2.0f * u2); n1 = rad * sinpif(2.0f * u2);
-      }
+      else jb_normal_pair(seed, stream_base + (uint64_t)m, ctr * 8 + (uint64_t)(a >> 1), n0, n1);
     }
     for (int q = 0; q < 2 && a + q < A; ++q) {
       const float mu = fminf(fmaxf(out[(size_t)m * nout + a + q], -5.f), 5.f);
