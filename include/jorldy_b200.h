@@ -164,6 +164,22 @@ JB_API int jb_ppo_loss(int continuous, const float* out, const int32_t* idx, con
                        void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * V-MPO (arXiv:1909.12238) minibatch loss on the PPO rollout path (csrc/vmpo.cu).  `out[B,nout]` holds the
+ * minibatch rows' head outputs (layout as for PPO), `out_old[NT,nout]` the pre-pass outputs of the whole rollout;
+ * out_old / action / adv / ret are gathered through idx (NULL: row b).  `mult` (device) = [eta, alpha_mu,
+ * alpha_sigma].  dout[B,nout] receives d loss / d out, dmult[3] d loss / d mult.  stats holds 16 + 4*ceil(B/256)
+ * floats: [0] actor_loss [1] critic_loss [2] eta_loss [3] alpha_loss [4] mean KL_mu (discrete: the KL)
+ * [5] mean KL_sigma [6] top-half size [7] median advantage; acc (may be NULL) accumulates [0..3] into acc[0..3]
+ * and counts minibatches in acc[4].  1 <= A <= 18 discrete, 1 <= A <= 8 continuous.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_vmpo_loss(int continuous, const float* out, const float* out_old, const int32_t* idx, const void* action,
+                        const float* adv, const float* ret, int B, int A, int nout, const float* mult, float eps_eta,
+                        float eps_alpha_mu, float eps_alpha_sigma, float* dout, float* dmult, float* stats, float* acc,
+                        void* stream);
+/* mult[k] = max(mult[k], minimum_k) after the multipliers' optimiser step */
+JB_API int jb_vmpo_clamp(float* mult, float min_eta, float min_alpha_mu, float min_alpha_sigma, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Synthetic Atari-shaped env — observation contract of jorldy/core/env/atari.py:56-61,112,145-160.
  * ------------------------------------------------------------------------------------------- */
 JB_API int jb_env_frames_reset(uint8_t* obs, int64_t* fcount, float* score, uint64_t seed, uint64_t stream_base, int n,

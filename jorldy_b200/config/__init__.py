@@ -5,7 +5,8 @@ config modules define (jorldy/config/<agent>/<env>.py: env / agent / optim / tra
 reference's shipped configs for the agents on the north-star path (dqn, double, dueling, multistep,
 per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, r2d2, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
-which follow the SAC-Discrete paper; an existing JORLDY config directory on sys.path takes precedence
+which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the V-MPO
+paper's multiplier settings; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -130,6 +131,33 @@ def _ppo_config(env):
                 train=dict(_TRAIN_SMALL, eval_iteration=10, distributed_batch_size=256, update_period=128, num_workers=8))
 
 
+# V-MPO (Song et al., ICLR 2020, arXiv:1909.12238), keys added to _ppo_config's row for the same env.  The values come
+# from the paper's hyper-parameter tables (Appendix): initial eta 1.0 in every table; discrete actions (DMLab / Atari
+# tables): initial alpha 5.0, eps_eta 0.01, eps_alpha in [0.005, 0.01] -> 0.01; continuous control table: initial
+# alpha_mu = alpha_sigma = 1.0, eps_eta 0.01, eps_alpha_mu in [0.005, 0.01] -> 0.005, eps_alpha_sigma in [5e-6, 5e-5]
+# -> 5e-5.  The minima are 1e-8 (the multipliers stay positive).  alpha_sigma / eps_alpha_sigma are unused by discrete
+# actions and kept at the continuous row's values.
+_VMPO_KEYS = dict(min_eta=1e-8, min_alpha_mu=1e-8, min_alpha_sigma=1e-8, eta=1.0, alpha_sigma=1.0, eps_eta=0.01,
+                  eps_alpha_sigma=5e-5)
+_VMPO_ENVS = ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")
+
+
+def _vmpo_config(env):
+    """V-MPO: PPO's config for the env (rollout, epochs, minibatch, GAE, clip_grad_norm, optimiser, train) plus the
+    multiplier keys above.  Not compared with the reference's config/vmpo/*.py, which takes precedence when a JORLDY
+    config directory is on sys.path."""
+    d = _ppo_config(env)
+    a = d["agent"]
+    for k in ("epsilon_clip", "vf_coef", "ent_coef"):      # PPO's loss coefficients: no V-MPO counterpart
+        a.pop(k)
+    a.update(_VMPO_KEYS, name="vmpo")
+    if a["network"].startswith("continuous"):
+        a.update(alpha_mu=1.0, eps_alpha_mu=0.005)
+    else:
+        a.update(alpha_mu=5.0, eps_alpha_mu=0.01)
+    return d
+
+
 # ---- continuous off-policy family: jorldy/config/{ddpg,td3,sac}/{cartpole,pendulum,mujoco}.py --------------------------------
 _TRAIN_MUJOCO = dict(training=True, load_path=None, run_step=1000000, print_period=10000, save_period=100000, eval_iteration=10)
 _AC_ENVS = {"ddpg": ("cartpole", "pendulum", "mujoco"), "td3": ("cartpole", "mujoco"), "sac": ("cartpole", "pendulum", "mujoco")}
@@ -201,6 +229,7 @@ def available():
     for ag in list(_VALUE_AGENTS) + ["ape_x", "r2d2"]:
         out += [f"config.{ag}.{e}" for e in ("cartpole", "mountaincar", "atari")]
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
+    out += [f"config.vmpo.{e}" for e in _VMPO_ENVS]
     return out
 
 
@@ -217,6 +246,8 @@ def load(config_path):
         d = _r2d2_config(env)
     elif agent == "ppo" and env in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari"):
         d = _ppo_config(env)
+    elif agent == "vmpo" and env in _VMPO_ENVS:
+        d = _vmpo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
     elif agent == "sac_discrete" and env in ("cartpole", "atari"):

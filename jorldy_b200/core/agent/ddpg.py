@@ -24,13 +24,15 @@ _DEFAULT_OPTIM = {"actor": "adam", "critic": "adam", "actor_lr": 5e-4, "critic_l
 
 
 class _Scalar(FlatNetwork):
-    """One learnable scalar (SAC's log_alpha, sac.py:95-100) held like a network so that the flat Adam applies."""
+    """Learnable scalars held like a network so that the flat Adam applies: SAC's log_alpha (sac.py:95-100), or V-MPO's
+    [eta, alpha_mu, alpha_sigma] as one contiguous vector when `value` is a sequence."""
 
     def __init__(self, name, value, device):
         super().__init__(device)
-        self._specs = [(name, (1,))]
+        values = [float(v) for v in np.atleast_1d(value)]
+        self._specs = [(name, (len(values),))]
         self._allocate()
-        self.flat[0] = value
+        self.flat[:len(values)] = torch.tensor(values, dtype=torch.float32)
 
 
 class _ActorCritic(BaseAgent):

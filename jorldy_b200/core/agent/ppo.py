@@ -146,10 +146,22 @@ class PPO(BaseAgent):
         self.optimizer.step(max_norm=self.clip_grad_norm)
 
     LAUNCHES_PER_MINIBATCH = 13   # take + in_fwd + gemm + heads + loss + finalize + 2 heads bwd + 3 gemm + sumsq + adam
+    _GRAPH_INPUTS = ("state", "action", "adv", "ret", "value", "logp_old", "perm")   # rollout tensors a graph reads
+
+    def _step_state(self):
+        """Every device tensor a minibatch step mutates (the graph warm-up saves and restores them)."""
+        return [self.network.flat, *self.optimizer.state_tensors(), self._acc, self._cursor]
+
+    def _begin_epochs(self):
+        """Device-side set-up before the optimisation epochs: the lr the graphs read and the learn accumulators."""
+        self.optimizer._sync_lr()          # graph replays do not pass through optimizer.step()'s host-side lr check
+        self._acc.zero_()
+        self._acc[3] = -float("inf")
+        self._acc[4] = float("inf")
 
     def _graph_for(self, st, B):
         """CUDA graph of GRAPH_CHUNK minibatch steps reading indices through the device cursor."""
-        key = (B,) + tuple(st[k].data_ptr() for k in ("state", "action", "adv", "ret", "value", "logp_old", "perm"))
+        key = (B,) + tuple(st[k].data_ptr() for k in self._GRAPH_INPUTS)
         g = self._graphs.get(key)
         if g is not None:
             return g
@@ -161,8 +173,7 @@ class PPO(BaseAgent):
                 self._minibatch_step(st, cur_idx, B)
 
         # warm-up on a side stream (allocates workspaces), restoring every mutated buffer afterwards
-        net, opt = self.network, self.optimizer
-        mutated = [net.flat, *opt.state_tensors(), self._acc, self._cursor]
+        mutated = self._step_state()
         saved = [t.clone() for t in mutated]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -229,10 +240,7 @@ class PPO(BaseAgent):
 
         # ---- optimisation epochs (ppo.py:114-175) ----
         B = self.batch_size
-        self.optimizer._sync_lr()          # graph replays do not pass through optimizer.step()'s host-side lr check
-        self._acc.zero_()
-        self._acc[3] = -float("inf")
-        self._acc[4] = float("inf")
+        self._begin_epochs()
         n_full = NT // B
         tail = NT - n_full * B
         from . import ppo_fused
@@ -266,7 +274,10 @@ class PPO(BaseAgent):
                            else n_steps * self.LAUNCHES_PER_MINIBATCH)
         n_chunks = (NT + 16383) // 16384
         self.n_prepass_launches = 3 * n_chunks + 1 + 3 + 1      # forward chunks + prepass + V(s') + gae
+        return self._learn_result(mean_ret)
 
+    def _learn_result(self, mean_ret):
+        """The result dict from the device accumulators and mean_ret, in one device->host read."""
         acc = torch.cat([self._acc[:6], mean_ret.view(1), self._acc[7:8]]).cpu().numpy()     # ONE device->host read
         if acc[7] != 0.0:
             dbg = [ws["partials"][200:205].tolist() for ws in (r.ws for r in self._fused.values())]

@@ -91,11 +91,13 @@ def attach(agent, world_size, average_with="avg"):
     rank 0) and an averaged flat gradient before every optimiser step."""
     if world_size <= 1:
         return agent
-    if hasattr(agent, "critics"):
-        # DDPG / TD3 / SAC (SURVEY 8f-4): several networks and optimisers per agent, no gradient exchange built for them —
-        # under torchrun every rank is an independent replica (own envs, own replay, own weights), and says so.
+    if hasattr(agent, "critics") or getattr(agent, "replicas_only", False):
+        # DDPG / TD3 / SAC (SURVEY 8f-4): several networks and optimisers per agent, no gradient exchange built for them;
+        # V-MPO: its median and psi normalisation are per minibatch, so an averaged sharded gradient is another algorithm.
+        # Under torchrun every rank is an independent replica (own envs, own replay, own weights), and says so.
         import warnings
-        warnings.warn(f"{type(agent).__name__}: replicas only (no data-parallel learner for the actor-critic family)")
+        family = "V-MPO" if getattr(agent, "replicas_only", False) else "the actor-critic family"
+        warnings.warn(f"{type(agent).__name__}: replicas only (no data-parallel learner for {family})")
         agent.world_size = 1
         return agent
     dist.broadcast(agent.network.flat, src=0)
