@@ -180,6 +180,55 @@ JB_API int jb_vmpo_loss(int continuous, const float* out, const float* out_old, 
 JB_API int jb_vmpo_clamp(float* mult, float min_eta, float min_alpha_mu, float min_alpha_sigma, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * ICM-PPO (Pathak et al., ICML 2017) on the PPO rollout path, csrc/icm.cu.  Column reductions split the rows into
+ * chunks of 256 and fold the chunks' float64 partial sums in chunk order; `partials` holds jb_col_partials_doubles(M, N)
+ * doubles.  No atomics anywhere: every entry point is bit-reproducible.
+ *   jb_bn_elu_fwd     y [M, ldy] (and y2 [M, ldy2] when not NULL) = ELU(BatchNorm1d(x)) with x [M, N] in training mode:
+ *                     biased batch variance, invstd = 1/sqrt(var + eps); mean / invstd [N] receive the batch statistics;
+ *                     running_mean / running_var (unbiased variance) updated with `momentum`, num_batches_tracked += 1.
+ *                     gamma NULL: y = ELU(x), no BatchNorm.  With BatchNorm, M < 2 is rejected (as torch does).
+ *   jb_bn_elu_bwd     dx [M, N] from dy [M, lddy] and the forward's output y [M, ldy]; with BatchNorm also dgamma, dbeta [N]
+ *                     (overwritten), from x, mean, invstd; xhat [M, N] is workspace.  gamma NULL: dx = dy ELU'.
+ *   jb_rms_update     OpenAI baselines' RunningMeanStd.update over the M rows of x [M, D]: float64 mean / var [D] and count,
+ *                     batch mean and population variance merged with the parallel formula.  D <= 1024.
+ *   jb_rms_normalize  y [M, D] = clip((x[idx[m]] - mean) / sqrt(var), +-clip) (idx NULL: row m); mean = var = NULL: a gather.
+ *   jb_icm_reward     normalize: per env the reward-forward filter rewems[n] = gamma rewems[n] + ri[n, t] over t (filt [N, T]
+ *                     receives the filtered values, rewems [N] persists), RunningMeanStd update of (rms_mean, rms_var,
+ *                     rms_count) with filt, then out = ext_coef reward + int_coef ri / (sqrt(rms_var) + 1e-7); without
+ *                     normalize out = ext_coef reward + int_coef ri.  reward / ri / out [N, T] actor-major.
+ *   jb_icm_loss       f [B, F] forward-model output, phi_next [B, ld_next] = phi(s'), g [B, A] inverse-model output,
+ *                     action gathered through idx (NULL: row b; int32 discrete, f32 [., A] continuous);
+ *                     ri [B] (may be NULL) = eta / 2 sum_F |f - phi_next|;  l_f = mean (f - phi_next)^2 over B F,
+ *                     df = beta d l_f / d f;  l_i = cross-entropy of softmax(g) (discrete, mean over B) or mean (g - a)^2
+ *                     over B A (continuous), dg = (1 - beta) d l_i / d g.  stats holds 4 + 3 ceil(B / 8) floats:
+ *                     [0] mean r_i [1] l_f [2] l_i [3] beta l_f + (1 - beta) l_i; acc (may be NULL) [0..2] += stats[0..2],
+ *                     acc[3] += 1.  df = dg = NULL: the reward-only pre-pass (ri required; g, action, stats unused).
+ *                     F = 256, 1 <= A <= 18 discrete, 1 <= A <= 8 continuous.
+ *   jb_icm_action_rows dst [M, ld] columns 0..A-1 = one-hot of action[idx[m]] (discrete) or the raw action (continuous).
+ *   jb_scale_f32      x *= s over n floats.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_col_partials_doubles(int M, int N);
+JB_API int jb_bn_elu_fwd(const float* x, int M, int N, const float* gamma, const float* beta, float* running_mean,
+                         float* running_var, int64_t* num_batches_tracked, float momentum, float eps, float* mean,
+                         float* invstd, double* partials, float* y, int ldy, float* y2, int ldy2, void* stream);
+JB_API int jb_bn_elu_bwd(const float* dy, int lddy, const float* y, int ldy, const float* x, int M, int N,
+                         const float* gamma, const float* mean, const float* invstd, float* xhat, double* partials,
+                         float* dx, float* dgamma, float* dbeta, void* stream);
+JB_API int jb_rms_update(const float* x, int M, int D, double* mean, double* var, double* count, double* partials,
+                         void* stream);
+JB_API int jb_rms_normalize(const float* x, const int32_t* idx, int M, int D, const double* mean, const double* var,
+                            float clip, float* y, void* stream);
+JB_API int jb_icm_reward(const float* reward, const float* ri, int N, int T, float gamma, int normalize, float* rewems,
+                         double* rms_mean, double* rms_var, double* rms_count, double* partials, float* filt,
+                         float ext_coef, float int_coef, float* out, void* stream);
+JB_API int jb_icm_loss(int continuous, const float* f, const float* phi_next, int ld_next, const float* g,
+                       const int32_t* idx, const void* action, int B, int A, int F, float eta, float beta, float* ri,
+                       float* df, float* dg, float* stats, float* acc, void* stream);
+JB_API int jb_icm_action_rows(int continuous, const void* action, const int32_t* idx, int M, int A, float* dst, int ld,
+                              void* stream);
+JB_API int jb_scale_f32(float* x, long long n, float s, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Synthetic Atari-shaped env — observation contract of jorldy/core/env/atari.py:56-61,112,145-160.
  * ------------------------------------------------------------------------------------------- */
 JB_API int jb_env_frames_reset(uint8_t* obs, int64_t* fcount, float* score, uint64_t seed, uint64_t stream_base, int n,

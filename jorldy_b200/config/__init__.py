@@ -6,7 +6,8 @@ reference's shipped configs for the agents on the north-star path (dqn, double, 
 per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, r2d2, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the V-MPO
-paper's multiplier settings; an existing JORLDY config directory on sys.path takes precedence
+paper's multiplier settings, and `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys;
+an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -158,6 +159,22 @@ def _vmpo_config(env):
     return d
 
 
+# ICM-PPO (Pathak et al., ICML 2017): keys added to _ppo_config's row for the same env, at the reference agent's
+# constructor defaults.  Atari: the CNN ICM, without observation normalisation (not implemented for frames).
+_ICM_PPO_KEYS = dict(icm_network="icm_mlp", beta=0.2, lamb=1.0, eta=0.01, extrinsic_coeff=1.0, intrinsic_coeff=1.0,
+                     obs_normalize=True, ri_normalize=True, batch_norm=True)
+_ICM_PPO_ENVS = ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")
+
+
+def _icm_ppo_config(env):
+    """ICM-PPO: PPO's config for the env plus the ICM keys above."""
+    d = _ppo_config(env)
+    d["agent"].update(_ICM_PPO_KEYS, name="icm_ppo")
+    if env == "atari":
+        d["agent"].update(icm_network="icm_cnn", obs_normalize=False)
+    return d
+
+
 # ---- continuous off-policy family: jorldy/config/{ddpg,td3,sac}/{cartpole,pendulum,mujoco}.py --------------------------------
 _TRAIN_MUJOCO = dict(training=True, load_path=None, run_step=1000000, print_period=10000, save_period=100000, eval_iteration=10)
 _AC_ENVS = {"ddpg": ("cartpole", "pendulum", "mujoco"), "td3": ("cartpole", "mujoco"), "sac": ("cartpole", "pendulum", "mujoco")}
@@ -230,6 +247,7 @@ def available():
         out += [f"config.{ag}.{e}" for e in ("cartpole", "mountaincar", "atari")]
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
     out += [f"config.vmpo.{e}" for e in _VMPO_ENVS]
+    out += [f"config.icm_ppo.{e}" for e in _ICM_PPO_ENVS]
     return out
 
 
@@ -248,6 +266,8 @@ def load(config_path):
         d = _ppo_config(env)
     elif agent == "vmpo" and env in _VMPO_ENVS:
         d = _vmpo_config(env)
+    elif agent == "icm_ppo" and env in _ICM_PPO_ENVS:
+        d = _icm_ppo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
     elif agent == "sac_discrete" and env in ("cartpole", "atari"):

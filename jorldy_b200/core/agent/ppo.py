@@ -191,8 +191,13 @@ class PPO(BaseAgent):
         self._graphs[key] = graph
         return graph
 
-    def _learn_tensors(self, state, action, reward, done, next_state=None, last_next_state=None):
-        """Everything is a device tensor; rows are actor-major [N*T, ...]."""
+    def _gae_reward(self, st, reward, next_state, N, T):
+        """The reward jb_gae reads.  next_state: the N*T next-state rows when the caller has them, else None."""
+        return reward
+
+    def _learn_tensors(self, state, action, reward, done, next_state=None, last_next_state=None, next_rows=None):
+        """Everything is a device tensor; rows are actor-major [N*T, ...].  next_rows: the N*T next states of a resident
+        rollout that keeps them (the reward hook reads them; V(s') still comes from last_next_state)."""
         net = self.network
         NT = state.shape[0]
         T = self.n_step
@@ -234,6 +239,7 @@ class PPO(BaseAgent):
             lv.copy_(lout[:, -1])
             nv = None
         # ---- GAE + returns + standardisation (ppo.py:95-110) ----
+        reward = self._gae_reward(st, reward, next_state if next_state is not None else next_rows, N, T)
         C.jb_gae(ptr(reward), ptr(done), ptr(st["value"]), ptr(nv), ptr(lv), N, T, self.gamma, self._lambda,
                  int(self.use_standardization), ptr(st["adv"]), ptr(st["ret"]), s)
         mean_ret = st["ret"].mean()
@@ -331,7 +337,7 @@ class PPO(BaseAgent):
             state, last = rollout.state.view(N * T, -1), rollout.last_next_state
         res = self._learn_tensors(state, rollout.action.view(N * T, -1) if self.continuous
                                   else rollout.action.view(N * T), rollout.reward.view(N * T),
-                                  rollout.done.view(N * T), last_next_state=last)
+                                  rollout.done.view(N * T), last_next_state=last, next_rows=rollout.next_rows())
         if frames:
             rollout.frames.check()      # after _learn_tensors' device->host read: no further wait
         rollout.clear()

@@ -30,6 +30,7 @@ class VMPO(PPO):
     LAUNCHES_PER_MINIBATCH = 16   # PPO's 13 with the V-MPO loss + finalize, plus the multipliers' sumsq + adam + clamp
     _GRAPH_INPUTS = PPO._GRAPH_INPUTS + ("out",)       # out: the pre-pass head outputs, the old policy of the KL terms
     replicas_only = True          # parallel.attach: the median and psi are per minibatch, an averaged shard gradient is not V-MPO
+    FAMILY = "V-MPO"
 
     def __init__(self, state_size, action_size, optim_config={"name": "adam"}, min_eta=1e-8, min_alpha_mu=1e-8,
                  min_alpha_sigma=1e-8, eps_eta=0.01, eps_alpha_mu=0.01, eps_alpha_sigma=5e-5, eta=1.0, alpha_mu=1.0,

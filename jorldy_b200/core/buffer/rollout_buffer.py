@@ -46,7 +46,10 @@ class RolloutBuffer(BaseBuffer):
 
 
 class DeviceRollout:
-    def __init__(self, num_envs, n_step, state_size, action_size, action_type, device=None):
+    """next_state=True keeps every step's next state in next_state [N, T, D] (the env's terminal observation at done
+    steps, not the post-reset one), for learners that read s' per row (ICM-PPO); otherwise only last_next_state."""
+
+    def __init__(self, num_envs, n_step, state_size, action_size, action_type, device=None, next_state=False):
         dev = require_cuda(device)
         N, T = num_envs, n_step
         self.N, self.T, self.device = N, T, dev
@@ -58,7 +61,12 @@ class DeviceRollout:
         self.reward = torch.zeros(N, T, dtype=torch.float32, device=dev)
         self.done = torch.zeros(N, T, dtype=torch.float32, device=dev)
         self.last_next_state = torch.zeros(N, state_size, dtype=torch.float32, device=dev)
+        self.next_state = torch.zeros(N, T, state_size, dtype=torch.float32, device=dev) if next_state else None
         self.t = 0
+
+    def next_rows(self):
+        """The N*T next states, actor-major, or None when the rollout does not keep them."""
+        return None if self.next_state is None else self.next_state.view(self.N * self.T, -1)
 
     def write(self, state, action, reward, done, next_state):
         t = self.t
@@ -69,6 +77,8 @@ class DeviceRollout:
             self.action[:, t].copy_(action.view(self.N, -1))
         self.reward[:, t].copy_(reward)
         self.done[:, t].copy_(done)
+        if self.next_state is not None:
+            self.next_state[:, t].copy_(next_state)
         if t == self.T - 1:
             self.last_next_state.copy_(next_state)
         self.t = t + 1
@@ -82,6 +92,8 @@ class DeviceRollout:
             self.action[:, t].copy_(action.view(self.N, -1))
         self.reward[:, t].copy_(reward)
         self.done[:, t].copy_(done)
+        if self.next_state is not None:
+            self.next_state[:, t].copy_(next_state)
         if t == self.T - 1:
             self.last_next_state.copy_(next_state)
         self.t = t + 1
@@ -99,9 +111,11 @@ class FrameRollout(DeviceRollout):
     into a per-env ring of frames_per_rollout(T) frames, and the rollout keeps int64 frame references instead of states:
     state_ref [N, T] and last_next_state [N] (the last step's next state).  That is 7-14 KB per env step on the ring
     against 28 KB as a uint8 stack and 113 KB as fp32.  action / reward / done are DeviceRollout's.  The learner reads
-    the states through `rows()` / `last_rows()` (buffer/frame_store.py FrameRows)."""
+    the states through `rows()` / `last_rows()` (buffer/frame_store.py FrameRows).  next_state=True also keeps every step's
+    next-state reference in next_ref [N, T] (the terminal stack at done steps), read through `next_rows()`; these stacks
+    lie in the same window of the ring as the states, so frames_per_rollout(T) keeps them resident too."""
 
-    def __init__(self, num_envs, n_step, action_size, action_type, device=None):
+    def __init__(self, num_envs, n_step, action_size, action_type, device=None, next_state=False):
         dev = require_cuda(device)
         N, T = num_envs, n_step
         self.N, self.T, self.device = N, T, dev
@@ -114,6 +128,8 @@ class FrameRollout(DeviceRollout):
         self.reward = torch.zeros(N, T, dtype=torch.float32, device=dev)
         self.done = torch.zeros(N, T, dtype=torch.float32, device=dev)
         self.last_next_state = torch.zeros(N, dtype=torch.int64, device=dev)
+        self.next_state = None
+        self.next_ref = torch.zeros(N, T, dtype=torch.int64, device=dev) if next_state else None
         self._refs = torch.zeros(2, N, dtype=torch.int64, device=dev)
         self.t = 0
 
@@ -126,6 +142,8 @@ class FrameRollout(DeviceRollout):
         returns the next state's reference, for write_after_step()."""
         s, x = self.frames.push(obs, next_obs, done, auto_reset, out=self._refs)
         self.state_ref[:, self.t].copy_(s)
+        if self.next_ref is not None:
+            self.next_ref[:, self.t].copy_(x)
         return x
 
     def rows(self):
@@ -134,3 +152,6 @@ class FrameRollout(DeviceRollout):
 
     def last_rows(self):
         return FrameRows(self.frames, self.last_next_state)
+
+    def next_rows(self):
+        return None if self.next_ref is None else FrameRows(self.frames, self.next_ref.view(-1))

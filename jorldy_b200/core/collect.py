@@ -17,10 +17,11 @@ class RolloutCollector:
         # Atari-shaped envs: every frame is pushed once and the rollout stores frame references (buffer/frame_store.py)
         self.frames = bool(getattr(env, "frame_stack", False))
         if self.frames:
-            self.rollout = FrameRollout(env.num_envs, self.T, env.action_size, env.action_type, device=agent.device)
+            self.rollout = FrameRollout(env.num_envs, self.T, env.action_size, env.action_type, device=agent.device,
+                                        next_state=getattr(agent, "needs_next_state", False))
         else:
             self.rollout = DeviceRollout(env.num_envs, self.T, env.state_size, env.action_size, env.action_type,
-                                         device=agent.device)
+                                         device=agent.device, next_state=getattr(agent, "needs_next_state", False))
         self.use_cuda_graph = use_cuda_graph
         self._graph = None
         # kernels of OUR library per env step: mlp_in_fwd + gemm + heads_fwd + act + env_step (the

@@ -70,9 +70,10 @@ class CNNHead:
             p[f"head.{name}.weight"].copy_(w.view(co, ci, k, k))
             p[f"head.{name}.bias"].zero_()
 
-    def forward(self, net, x, idx, M, tag, save):
+    def forward(self, net, x, idx, M, tag, save, out=None):
         """x: a tensor of stacks, or a frame-ring row source (buffer/frame_store.py FrameRows) whose im2col fills conv1's
-        column matrix straight from the ring; rows idx[M] (int32) or all of them."""
+        column matrix straight from the ring; rows idx[M] (int32) or all of them.  out: [M, D_head_out] destination (None:
+        the tag's workspace)."""
         rows = None if torch.is_tensor(x) else x
         if rows is not None and self.D_in != tuple(rows.shape[1:]):
             raise ValueError(f"a frame-ring input is {tuple(rows.shape[1:])}, this head takes {self.D_in}")
@@ -98,7 +99,7 @@ class CNNHead:
                             M * oh * ow, K, co, 1, s)
             cur = y
         P = self.d3[0] * self.d3[1]
-        feat = net._buf(tag + "head.h", (M, self.D_head_out))
+        feat = out if out is not None else net._buf(tag + "head.h", (M, self.D_head_out))
         C.jb_nhwc_to_nchw(ptr(cur), M, P, 64, ptr(feat), s)
         return feat
 

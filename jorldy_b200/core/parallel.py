@@ -93,10 +93,11 @@ def attach(agent, world_size, average_with="avg"):
         return agent
     if hasattr(agent, "critics") or getattr(agent, "replicas_only", False):
         # DDPG / TD3 / SAC (SURVEY 8f-4): several networks and optimisers per agent, no gradient exchange built for them;
-        # V-MPO: its median and psi normalisation are per minibatch, so an averaged sharded gradient is another algorithm.
+        # V-MPO: its median and psi normalisation are per minibatch, so an averaged sharded gradient is another algorithm;
+        # ICM-PPO: its BatchNorm batch statistics and its observation / intrinsic-reward running statistics are per replica.
         # Under torchrun every rank is an independent replica (own envs, own replay, own weights), and says so.
         import warnings
-        family = "V-MPO" if getattr(agent, "replicas_only", False) else "the actor-critic family"
+        family = agent.FAMILY if getattr(agent, "replicas_only", False) else "the actor-critic family"
         warnings.warn(f"{type(agent).__name__}: replicas only (no data-parallel learner for {family})")
         agent.world_size = 1
         return agent
