@@ -180,6 +180,44 @@ JB_API int jb_vmpo_loss(int continuous, const float* out, const float* out_old, 
 JB_API int jb_vmpo_clamp(float* mult, float min_eta, float min_alpha_mu, float min_alpha_sigma, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * MPO (arXiv:1806.06920) on the replay path, csrc/mpo.cu: Retrace targets (arXiv:1606.02647) over B stored windows of
+ * n <= 32 steps, the sampled E-step and the decoupled-KL M-step (arXiv:1812.02256) with mult = [eta, alpha_mu,
+ * alpha_sigma] on the device.  Head rows are PPO's without the value: discrete logits [A] (A <= 18), continuous raw
+ * [mu | log_std] [2A] (A <= 8).  State rows of window b are b*(n+1) + t (t = 0..n), step rows b*n + t (t < n).
+ *   jb_mpo_logp           logp[M] = log pi(action | out) (discrete: int64 actions, continuous: the Normal log-pdf of
+ *                         atanh(clamp(a, +-(1-1e-7))) summed over dims, no Jacobian); out rows nout apart
+ *   jb_mpo_sample         for R target-actor rows raw [R, 2A] and normals eps [R, K, A] (K <= 64): z = mu + sd eps
+ *                         [R, K, A]; the critic input xs [R*KK, D] (each state row x [R, D] repeated KK times) and
+ *                         as [R*KK, A] = tanh(z) for k < K; with `taken` [B*n, A] (R = B*(n+1)), KK = K + 1 and slot K
+ *                         holds the taken action a_t (0 at t = n), else KK = K
+ *   jb_mpo_critic_target  tq: target critic, discrete [B*(n+1), A], continuous [B*(n+1)*(K+1)] (the K samples, then the
+ *                         taken action); tout [B*(n+1), nout] the target actor; q the online critic, discrete [B*n, A],
+ *                         continuous [B*n]; action int64 [B*n] / f32 [B*n, A]; log_mu, reward, done [B*n].
+ *                         V'_t = E_pi' Q'(s_t, .) (continuous: the mean of the K samples), c_t = min(1, pi'(a_t)/mu_t)
+ *                         (retrace = 0: c_t = 0), Qret_{n-1} = r + gamma (1-d) V'_n,
+ *                         Qret_t = r_t + gamma (1-d_t) [V'_{t+1} + c_{t+1} (Qret_{t+1} - Q'(s_{t+1}, a_{t+1}))];
+ *                         qret [B*n], dq = 2 (Q - Qret) / (B n) (discrete: in the taken action's column, 0 elsewhere);
+ *                         stats[0] = mean (Q - Qret)^2, stats[1] = mean Qret.  One CTA, fixed-order sums.
+ *   jb_mpo_policy_loss    over the S = B*n states: q(a) ∝ pi'(a) exp(Q'/eta) (discrete, exact) or softmax_k Q'(a_k)/eta
+ *                         (continuous, z [B*(n+1), K, A] from jb_mpo_sample); L_eta, L_pi, KL(pi' || pi) (discrete) or
+ *                         the decoupled KL_mu / KL_sigma, L_alpha; dout [S, nout] = d loss / d out, dmult[3];
+ *                         stats[0..4] = L_pi, L_eta, L_alpha, mean KL_mu, mean KL_sigma; partials holds
+ *                         jb_mpo_policy_partials(S) floats, folded in CTA order by a one-thread launch.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_mpo_logp(int continuous, const float* out, int nout, const void* action, int M, int A, float* logp,
+                       void* stream);
+JB_API int jb_mpo_sample(const float* raw, const float* eps, int R, int K, int A, const float* x, int D, const float* taken,
+                         int n, float* z, float* xs, float* as, void* stream);
+JB_API int jb_mpo_critic_target(int continuous, const float* tq, const float* tout, const float* q, const void* action,
+                                const float* log_mu, const float* reward, const float* done, int B, int n, int A, int K,
+                                float gamma, int retrace, float* dq, float* qret, float* stats, void* stream);
+JB_API int jb_mpo_policy_partials(int S);
+JB_API int jb_mpo_policy_loss(int continuous, const float* out, const float* tout, const float* tq, const float* z, int B,
+                              int n, int A, int K, const float* mult, float eps_eta, float eps_alpha_mu,
+                              float eps_alpha_sigma, float* dout, float* dmult, float* partials, float* stats,
+                              void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * ICM-PPO (Pathak et al., ICML 2017) on the PPO rollout path, csrc/icm.cu.  Column reductions split the rows into
  * chunks of 256 and fold the chunks' float64 partial sums in chunk order; `partials` holds jb_col_partials_doubles(M, N)
  * doubles.  No atomics anywhere: every entry point is bit-reproducible.

@@ -6,8 +6,8 @@ reference's shipped configs for the agents on the north-star path (dqn, double, 
 per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, r2d2, ppo, and ddpg / td3 / sac of SURVEY 8f-4) on cartpole / mountaincar /
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the V-MPO
-paper's multiplier settings, and `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys;
-an existing JORLDY config directory on sys.path takes precedence
+paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys,
+and `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -238,6 +238,34 @@ def _sac_discrete_config(env):
                 train=dict(_TRAIN_ATARI, update_period=4, num_workers=16))
 
 
+# MPO (arXiv:1806.06920): this project's choices, not a reference config file.  The agent keys are shared by every env
+# (V-MPO's constructor defaults for the multipliers); buffer_size / start_train_step and the train dict are SAC's for
+# the same env (mountaincar: cartpole's replay keys and the value agents' _TRAIN_SMALL row).
+_MPO_KEYS = dict(name="mpo", hidden_size=512, gamma=0.99, n_step=8, batch_size=64, critic_loss_type="retrace", num_sample=30,
+                 target_update_period=100, clip_grad_norm=1.0, min_eta=1e-8, min_alpha_mu=1e-8, min_alpha_sigma=1e-8,
+                 eps_eta=0.01, eps_alpha_mu=0.01, eps_alpha_sigma=5e-5, eta=1.0, alpha_mu=1.0, alpha_sigma=1.0, lr_decay=True)
+_MPO_ENVS = ("cartpole", "mountaincar", "pendulum", "mujoco")
+
+
+def _mpo_config(env):
+    """MPO: discrete_policy / discrete_q_network on cartpole and mountaincar, continuous_policy / continuous_q_network on
+    pendulum and mujoco; one Adam setting (lr 3e-4) for the actor, the critic and the multipliers.  These are this
+    project's choices; a JORLDY config directory on sys.path takes precedence."""
+    sac = _ac_config("sac", "cartpole" if env == "mountaincar" else env)
+    a = dict(_MPO_KEYS, buffer_size=sac["agent"]["buffer_size"], start_train_step=sac["agent"]["start_train_step"])
+    if env in ("cartpole", "mountaincar"):
+        a.update(actor="discrete_policy", critic="discrete_q_network")
+    else:
+        a.update(actor="continuous_policy", critic="continuous_q_network")
+    if env == "cartpole":
+        env_d, tr = dict(name="cartpole", action_type="discrete", render=False), sac["train"]
+    elif env == "mountaincar":
+        env_d, tr = dict(name="mountain_car", render=False), dict(_TRAIN_SMALL, eval_iteration=10, update_period=32, num_workers=8)
+    else:
+        env_d, tr = sac["env"], sac["train"]
+    return dict(env=env_d, agent=a, optim=dict(name="adam", lr=3e-4), train=tr)
+
+
 def available():
     out = []
     for ag, envs in _AC_ENVS.items():
@@ -248,6 +276,7 @@ def available():
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
     out += [f"config.vmpo.{e}" for e in _VMPO_ENVS]
     out += [f"config.icm_ppo.{e}" for e in _ICM_PPO_ENVS]
+    out += [f"config.mpo.{e}" for e in _MPO_ENVS]
     return out
 
 
@@ -268,6 +297,8 @@ def load(config_path):
         d = _vmpo_config(env)
     elif agent == "icm_ppo" and env in _ICM_PPO_ENVS:
         d = _icm_ppo_config(env)
+    elif agent == "mpo" and env in _MPO_ENVS:
+        d = _mpo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
     elif agent == "sac_discrete" and env in ("cartpole", "atari"):

@@ -84,41 +84,56 @@ class VMPO(PPO):
         super().learning_rate_decay(step, [self.optimizer, self.mult_optimizer] if optimizers is None else optimizers, mode)
 
     # ------------------------------------------------------------------------------ checkpoint --
-    # One torch-Adam layout over network.parameters() + [eta, alpha_mu, alpha_sigma]: the multipliers are the three
-    # parameter indices after the network's, each a 0-d tensor; their values are stored under their own names too.
     def save(self, path):
         print(f"...Save model to {path}...")
-        sd = cpu_optimizer_state(self.optimizer)
-        P = len(self.network.p)
-        step = float(self.mult_optimizer._step_dev.item())
-        if step > 0:
-            m, v = self.mult_optimizer.exp_avg[:3].cpu(), self.mult_optimizer.exp_avg_sq[:3].cpu()
-            for k in range(3):
-                sd["state"][P + k] = {"step": torch.tensor(step), "exp_avg": m[k].clone(), "exp_avg_sq": v[k].clone()}
-        sd["param_groups"][0]["params"] = list(range(P + 3))
-        vals = self.mult.flat[:3].cpu()
-        ck = {"network": cpu_state_dict(self.network), "optimizer": sd}
-        ck.update({name: vals[k].clone() for k, name in enumerate(MULTIPLIERS)})
+        ck = {"network": cpu_state_dict(self.network), "optimizer": joint_optimizer_state(self.optimizer, self.mult_optimizer)}
+        ck.update(multiplier_values(self.mult))
         torch.save(ck, os.path.join(path, "ckpt"))
 
     def load(self, path):
         print(f"...Load model from {path}...")
         ck = torch.load(os.path.join(path, "ckpt"), map_location="cpu", weights_only=False)
         self.network.load_state_dict(ck["network"])
-        P = len(self.network.p)
-        sd = ck["optimizer"]
-        st = sd.get("state", {})
-        get = lambda i: st[i] if i in st else st.get(str(i))
-        group = dict(sd["param_groups"][0], params=list(range(P)))
-        self.optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {}, "param_groups": [group]})
-        self.mult_optimizer.param_groups[0]["lr"] = float(group["lr"])
-        if get(P) is not None:
-            opt = self.mult_optimizer
-            for k in range(3):
-                e = get(P + k)
-                opt.exp_avg[k].copy_(torch.as_tensor(e["exp_avg"]).reshape(()))
-                opt.exp_avg_sq[k].copy_(torch.as_tensor(e["exp_avg_sq"]).reshape(()))
-            opt._step_dev.fill_(int(float(get(P)["step"])))
-        for k, name in enumerate(MULTIPLIERS):
-            if name in ck:
-                self.mult.flat[k].copy_(torch.as_tensor(ck[name], dtype=torch.float32).reshape(()))
+        load_joint_optimizer_state(ck["optimizer"], self.optimizer, self.mult_optimizer)
+        load_multipliers(ck, self.mult)
+
+
+# One torch-Adam layout over network.parameters() + [eta, alpha_mu, alpha_sigma]: the multipliers are the three parameter
+# indices after the network's, each a 0-d tensor; their values are stored under their own names too.  V-MPO's and MPO's
+# checkpoints share it.
+def joint_optimizer_state(optimizer, mult_optimizer):
+    sd = cpu_optimizer_state(optimizer)
+    P = len(optimizer.network.p)
+    step = float(mult_optimizer._step_dev.item())
+    if step > 0:
+        m, v = mult_optimizer.exp_avg[:3].cpu(), mult_optimizer.exp_avg_sq[:3].cpu()
+        for k in range(3):
+            sd["state"][P + k] = {"step": torch.tensor(step), "exp_avg": m[k].clone(), "exp_avg_sq": v[k].clone()}
+    sd["param_groups"][0]["params"] = list(range(P + 3))
+    return sd
+
+
+def multiplier_values(mult):
+    vals = mult.flat[:3].cpu()
+    return {name: vals[k].clone() for k, name in enumerate(MULTIPLIERS)}
+
+
+def load_joint_optimizer_state(sd, optimizer, mult_optimizer):
+    P = len(optimizer.network.p)
+    st = sd.get("state", {})
+    get = lambda i: st[i] if i in st else st.get(str(i))
+    group = dict(sd["param_groups"][0], params=list(range(P)))
+    optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {}, "param_groups": [group]})
+    mult_optimizer.param_groups[0]["lr"] = float(group["lr"])
+    if get(P) is not None:
+        for k in range(3):
+            e = get(P + k)
+            mult_optimizer.exp_avg[k].copy_(torch.as_tensor(e["exp_avg"]).reshape(()))
+            mult_optimizer.exp_avg_sq[k].copy_(torch.as_tensor(e["exp_avg_sq"]).reshape(()))
+        mult_optimizer._step_dev.fill_(int(float(get(P)["step"])))
+
+
+def load_multipliers(ck, mult):
+    for k, name in enumerate(MULTIPLIERS):
+        if name in ck:
+            mult.flat[k].copy_(torch.as_tensor(ck[name], dtype=torch.float32).reshape(()))

@@ -73,10 +73,14 @@ class NStepAssembler:
     n steps, next_state = last step's next_state) and ape_x.py:174-199 (window of n+1, next_state = the
     (n+1)-th step's state, actor-side priority |G_n - q_0|) — including their behaviour of NOT clearing at
     episode ends (windows straddle episodes and rely on the (1-done) mask).  One ring [N, L, ...] per field.
+
+    trajectory=True emits the whole window instead (MPO's Retrace learner): state [N, n+1, ...] (s_0 .. s_{n-1} and the
+    last step's next_state), and action, reward, done, log_mu [N, n, ...], oldest step first.  Inside a window s_{t+1}
+    is the next state of step t wherever done_t = 0, so no per-step next_state is stored.
     """
 
-    def __init__(self, n_step, apex=False, gamma=0.99):
-        self.n, self.apex, self.gamma = n_step, apex, gamma
+    def __init__(self, n_step, apex=False, gamma=0.99, trajectory=False):
+        self.n, self.apex, self.gamma, self.trajectory = n_step, apex, gamma, trajectory
         self.L = n_step + 1 if apex else n_step
         self.hist, self.count, self.pos = None, 0, 0
 
@@ -95,6 +99,11 @@ class NStepAssembler:
         oldest = self.pos                  # after the increment, pos points at the oldest entry
         order = [(oldest + i) % self.L for i in range(self.L)]
         h = self.hist
+        if self.trajectory:
+            sel = torch.as_tensor(order, device=h["reward"].device)
+            out = {k: h[k].index_select(1, sel) for k in ("action", "reward", "done", "log_mu")}
+            out["state"] = torch.cat([h["state"].index_select(1, sel), h["next_state"][:, newest:newest + 1]], dim=1)
+            return out
         out = {"state": h["state"][:, oldest].clone(), "action": h["action"][:, oldest].clone()}
         if self.apex:
             out["next_state"] = h["state"][:, newest].clone()
@@ -168,9 +177,11 @@ class ReplayCollector:
         self.env, self.agent, self.update_period = env, agent, update_period
         n = getattr(agent, "n_step", 1)
         apex = type(agent).__name__ == "ApeX"
+        trajectory = getattr(agent, "trajectory_windows", False)      # MPO: whole windows with the behaviour log mu
         # recurrent agents (R2D2) bring their own sequence assembler and frame store
         self.sequences = getattr(agent, "sequence_assembler", None)
-        self.assembler = NStepAssembler(n, apex, agent.gamma) if (n > 1 or apex) and self.sequences is None else None
+        self.assembler = NStepAssembler(n, apex, agent.gamma, trajectory) \
+            if (n > 1 or apex or trajectory) and self.sequences is None else None
         if apex or self.sequences is not None:
             agent.set_actor_epsilons(env.num_envs, total=max(agent.num_workers, env.num_envs, 2))
         env.reset_device()
@@ -206,6 +217,8 @@ class ReplayCollector:
             if self.assembler is not None:
                 if self.assembler.apex:
                     tr["q"] = q_sel.clone()
+                if self.assembler.trajectory:
+                    tr["log_mu"] = q_sel.view(-1).clone()
                 out = self.assembler.push({k: (v.view(v.shape[0]) if k in ("reward", "done") else v) for k, v in tr.items()})
                 if out is not None:
                     batches.append(out)
