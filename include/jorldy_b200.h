@@ -137,6 +137,15 @@ JB_API int jb_heads_bwd_dx(const float* dout, const float* h, int M, int H, cons
                            int n1, const float* w2, int n2, float* dh, void* stream);
 JB_API int jb_heads_bwd_dw(const float* dout, const float* h, int M, int H, float* dw0, float* db0, int n0, float* dw1,
                            float* db1, int n1, float* dw2, float* db2, int n2, void* stream);
+/* The same layers over an array of 1 <= n_heads <= 4 heads (host arrays of device pointers and widths, sum(n) <= 32):
+ * head g has weight w[g] [n[g], H] and bias b[g] [n[g]], out is [M, sum(n)].  The three-head entry points above are
+ * these calls with n_heads = 3. */
+JB_API int jb_heads_fwd_n(const float* h, int M, int H, int n_heads, const float* const* w, const float* const* b,
+                          const int* n, float* out, void* stream);
+JB_API int jb_heads_bwd_dx_n(const float* dout, const float* h, int M, int H, int n_heads, const float* const* w,
+                             const int* n, float* dh, void* stream);
+JB_API int jb_heads_bwd_dw_n(const float* dout, const float* h, int M, int H, int n_heads, float* const* dw,
+                             float* const* db, const int* n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * PPO — jorldy/core/agent/ppo.py:54-69 (act), :83-93 (value / log_prob_old), :127-162 (loss).
@@ -216,6 +225,39 @@ JB_API int jb_mpo_policy_loss(int continuous, const float* out, const float* tou
                               int n, int A, int K, const float* mult, float eps_eta, float eps_alpha_mu,
                               float eps_alpha_sigma, float* dout, float* dmult, float* partials, float* stats,
                               void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * RND-PPO (Burda et al., arXiv:1810.12894) on the PPO rollout path, csrc/rnd.cu.  The policy network has a second value
+ * head: `out[M,nout]` is discrete [logits(A)|v|v_i] (nout = A + 2) or continuous [mu(A)|log_std(A)|v|v_i]
+ * (nout = 2A + 2).  1 <= A <= 18 discrete, 1 <= A <= 8 continuous.  No atomics: every entry point is bit-reproducible.
+ *   jb_rnd_prepass    value [M], value_i [M] and logp_old (discrete [M], continuous [M, A]) of the pre-pass rows, with
+ *                     PPO's pre-pass log-prob.
+ *   jb_rnd_ppo_loss   jb_ppo_loss with a second clipped critic: critic_loss = max(mse(v, ret), mse(v_clip, ret))
+ *                     + max(mse(v_i, ret_i), mse(v_i_clip, ret_i)), each stream clipped around its own old value;
+ *                     loss = actor + vf_coef critic + ent_coef entropy.  ret_i / value_i_old are full-rollout arrays
+ *                     gathered through idx like the others.  dout [B, nout].  stats holds 8 + 4*ceil(B/256) floats:
+ *                     [0] actor_loss [1] critic_loss [2] entropy_loss [3] max_ratio [4] min_prob [5] extrinsic critic
+ *                     [6] intrinsic critic [7] 0; acc (may be NULL) accumulates [0..4] and counts in acc[5] as jb_ppo_loss
+ *                     does.  With ret_i = value_i = value_i_old the policy and v columns of dout and stats[0..4] equal
+ *                     jb_ppo_loss's bit for bit.
+ *   jb_rnd_loss       p [B, F] predictor output, target [rows, F] the cached target features read at idx[b] (NULL: b);
+ *                     ri [B] (may be NULL) = mean_F (p - target)^2; dp [B, F] = d rnd_loss / d p with
+ *                     rnd_loss = mean_B ri.  stats holds 1 + ceil(B / 8) floats: [0] rnd_loss; acc (may be NULL)
+ *                     acc[0] += rnd_loss, acc[1] += 1.  dp = NULL: the reward-only pre-pass (ri required, stats unused).
+ *                     F = 256.
+ *   jb_adv_mix        adv [N, T] = ext_coef adv_e + int_coef adv_i, then with `standardize` each row standardised as
+ *                     jb_gae does it ((adv - mean) / (std + 1e-7), unbiased std, float64 sums in jb_gae's order).
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_rnd_prepass(int continuous, const float* out, const void* action, int M, int A, int nout, float* value,
+                          float* value_i, float* logp_old, void* stream);
+JB_API int jb_rnd_ppo_loss(int continuous, const float* out, const int32_t* idx, const void* action, const float* adv,
+                           const float* ret, const float* value_old, const float* ret_i, const float* value_i_old,
+                           const float* logp_old, int B, int A, int nout, float eps_clip, float vf_coef, float ent_coef,
+                           float* dout, float* stats, float* acc, void* stream);
+JB_API int jb_rnd_loss(const float* p, const float* target, const int32_t* idx, int B, int F, float* ri, float* dp,
+                       float* stats, float* acc, void* stream);
+JB_API int jb_adv_mix(const float* adv_e, const float* adv_i, int N, int T, float ext_coef, float int_coef,
+                      int standardize, float* adv, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ICM-PPO (Pathak et al., ICML 2017) on the PPO rollout path, csrc/icm.cu.  Column reductions split the rows into

@@ -7,6 +7,7 @@ per, noisy, c51, rainbow, qrdqn, iqn, m_dqn, m_iqn, rainbow_iqn, ape_x, r2d2, pp
 pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action SAC's `config.sac_discrete.{cartpole,atari}` (agent name "sac"),
 which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the V-MPO
 paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys,
+`config.rnd_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the RND keys,
 and `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
@@ -175,6 +176,22 @@ def _icm_ppo_config(env):
     return d
 
 
+# RND-PPO (Burda et al., arXiv:1810.12894): keys added to _ppo_config's row for the same env, with the paper's advantage
+# weights (extrinsic 2, intrinsic 1).  Atari: the CNN RND, without observation normalisation (not implemented for frames).
+_RND_PPO_KEYS = dict(rnd_network="rnd_mlp", gamma_i=0.99, extrinsic_coeff=2.0, intrinsic_coeff=1.0, obs_normalize=True,
+                     ri_normalize=True, batch_norm=True, non_episodic=True)
+_RND_PPO_ENVS = ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")
+
+
+def _rnd_ppo_config(env):
+    """RND-PPO: PPO's config for the env plus the RND keys above."""
+    d = _ppo_config(env)
+    d["agent"].update(_RND_PPO_KEYS, name="rnd_ppo")
+    if env == "atari":
+        d["agent"].update(rnd_network="rnd_cnn", obs_normalize=False)
+    return d
+
+
 # ---- continuous off-policy family: jorldy/config/{ddpg,td3,sac}/{cartpole,pendulum,mujoco}.py --------------------------------
 _TRAIN_MUJOCO = dict(training=True, load_path=None, run_step=1000000, print_period=10000, save_period=100000, eval_iteration=10)
 _AC_ENVS = {"ddpg": ("cartpole", "pendulum", "mujoco"), "td3": ("cartpole", "mujoco"), "sac": ("cartpole", "pendulum", "mujoco")}
@@ -276,6 +293,7 @@ def available():
     out += [f"config.ppo.{e}" for e in ("cartpole", "mountaincar", "pendulum", "mujoco", "atari")]
     out += [f"config.vmpo.{e}" for e in _VMPO_ENVS]
     out += [f"config.icm_ppo.{e}" for e in _ICM_PPO_ENVS]
+    out += [f"config.rnd_ppo.{e}" for e in _RND_PPO_ENVS]
     out += [f"config.mpo.{e}" for e in _MPO_ENVS]
     return out
 
@@ -297,6 +315,8 @@ def load(config_path):
         d = _vmpo_config(env)
     elif agent == "icm_ppo" and env in _ICM_PPO_ENVS:
         d = _icm_ppo_config(env)
+    elif agent == "rnd_ppo" and env in _RND_PPO_ENVS:
+        d = _rnd_ppo_config(env)
     elif agent == "mpo" and env in _MPO_ENVS:
         d = _mpo_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:

@@ -24,22 +24,11 @@ import torch
 from ..dev import C, ptr, stream_ptr
 from ..network.icm import FEATURE, ICM_MLP
 from ..optimizer import Optimizer
-from .base import cpu_optimizer_state, cpu_state_dict
+from .base import cpu_state_dict
+from .curiosity import _RunningMeanStd, check_batch_norm_rows, load_two_adam_state, two_adam_state
 from .ppo import PPO
 
 ICM_NETWORKS = {"icm_mlp": "mlp", "icm_cnn": "cnn"}       # ICM network -> the policy head (observation kind) it pairs with
-
-
-class _RunningMeanStd:
-    """OpenAI baselines' RunningMeanStd on the device: float64 mean / var, count starting at 1e-4."""
-
-    def __init__(self, shape, device):
-        self.mean = torch.zeros(shape, dtype=torch.float64, device=device)
-        self.var = torch.ones(shape, dtype=torch.float64, device=device)
-        self.count = torch.full((1,), 1e-4, dtype=torch.float64, device=device)
-
-    def tensors(self):
-        return [self.mean, self.var, self.count]
 
 
 class ICM_PPO(PPO):
@@ -77,10 +66,7 @@ class ICM_PPO(PPO):
 
     # ----------------------------------------------------------------------------------- learn --
     def _check_batch(self, NT):
-        B = self.batch_size
-        if self.batch_norm and (B < 2 or NT % B == 1):
-            raise ValueError(f"ICM-PPO with batch_norm: a minibatch of one row cannot be batch-normalised "
-                             f"(batch_size={B}, rollout of {NT} rows); choose batch_size >= 2 with rollout % batch_size != 1")
+        check_batch_norm_rows(self.FAMILY, self.batch_norm, self.batch_size, NT)
 
     def _gae_reward(self, st, reward, next_state, N, T):
         NT = N * T
@@ -179,13 +165,8 @@ class ICM_PPO(PPO):
     # network / icm / optimizer, the optimizer one torch-Adam layout over network.parameters() + icm.parameters().
     def save(self, path):
         print(f"...Save model to {path}...")
-        sd = cpu_optimizer_state(self.optimizer)
-        isd = cpu_optimizer_state(self.icm_optimizer)
-        P = len(self.network.p)
-        for i, e in isd["state"].items():
-            sd["state"][P + i] = e
-        sd["param_groups"][0]["params"] = list(range(P + len(self.icm.p)))
-        ck = {"network": cpu_state_dict(self.network), "icm": cpu_state_dict(self.icm), "optimizer": sd}
+        ck = {"network": cpu_state_dict(self.network), "icm": cpu_state_dict(self.icm),
+              "optimizer": two_adam_state(self.optimizer, self.icm_optimizer)}
         torch.save(ck, os.path.join(path, "ckpt"))
 
     def load(self, path):
@@ -193,12 +174,4 @@ class ICM_PPO(PPO):
         ck = torch.load(os.path.join(path, "ckpt"), map_location="cpu", weights_only=False)
         self.network.load_state_dict(ck["network"])
         self.icm.load_state_dict(ck["icm"])
-        P, Q = len(self.network.p), len(self.icm.p)
-        sd = ck["optimizer"]
-        st = sd.get("state", {})
-        get = lambda i: st[i] if i in st else st.get(str(i))
-        group = dict(sd["param_groups"][0])
-        self.optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {},
-                                        "param_groups": [dict(group, params=list(range(P)))]})
-        self.icm_optimizer.load_state_dict({"state": {i: get(P + i) for i in range(Q)} if get(P) is not None else {},
-                                            "param_groups": [dict(group, params=list(range(Q)))]})
+        load_two_adam_state(ck["optimizer"], self.optimizer, self.icm_optimizer)

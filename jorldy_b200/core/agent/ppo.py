@@ -195,29 +195,12 @@ class PPO(BaseAgent):
         """The reward jb_gae reads.  next_state: the N*T next-state rows when the caller has them, else None."""
         return reward
 
-    def _learn_tensors(self, state, action, reward, done, next_state=None, last_next_state=None, next_rows=None):
-        """Everything is a device tensor; rows are actor-major [N*T, ...].  next_rows: the N*T next states of a resident
-        rollout that keeps them (the reward hook reads them; V(s') still comes from last_next_state)."""
+    def _advantages(self, st, state, action, reward, done, next_state, last_next_state, next_rows, N, T):
+        """The pre-pass, V(s'), GAE and returns into st (value, logp_old, adv, ret); returns mean_ret on the device."""
         net = self.network
-        NT = state.shape[0]
-        T = self.n_step
-        N = NT // T
-        assert N * T == NT, f"rollout of {NT} rows is not a multiple of n_step={T} (ppo.py:97 view(-1, n_step) would raise)"
+        NT = N * T
         A = self.action_size
-        dev = self.device
         s = stream_ptr()
-        st = getattr(self, "_st", None)
-        if st is None or st["NT"] != NT:
-            st = {"NT": NT,
-                  "out": torch.empty(NT, net.nout, device=dev),
-                  "value": torch.empty(NT, device=dev),
-                  "logp_old": torch.empty(NT, A if self.continuous else 1, device=dev),
-                  "adv": torch.empty(NT, device=dev), "ret": torch.empty(NT, device=dev),
-                  "next_value": torch.empty(NT, device=dev),
-                  "perm": torch.empty(NT, dtype=torch.int32, device=dev)}
-            self._st = st
-        st["state"] = state
-        st["action"] = action
         # ---- pre-pass: value and log_prob_old (ppo.py:83-93) ----
         net.forward_rows(state, st["out"])
         if self.continuous:
@@ -242,7 +225,31 @@ class PPO(BaseAgent):
         reward = self._gae_reward(st, reward, next_state if next_state is not None else next_rows, N, T)
         C.jb_gae(ptr(reward), ptr(done), ptr(st["value"]), ptr(nv), ptr(lv), N, T, self.gamma, self._lambda,
                  int(self.use_standardization), ptr(st["adv"]), ptr(st["ret"]), s)
-        mean_ret = st["ret"].mean()
+        return st["ret"].mean()
+
+    def _learn_tensors(self, state, action, reward, done, next_state=None, last_next_state=None, next_rows=None):
+        """Everything is a device tensor; rows are actor-major [N*T, ...].  next_rows: the N*T next states of a resident
+        rollout that keeps them (the reward hook reads them; V(s') still comes from last_next_state)."""
+        net = self.network
+        NT = state.shape[0]
+        T = self.n_step
+        N = NT // T
+        assert N * T == NT, f"rollout of {NT} rows is not a multiple of n_step={T} (ppo.py:97 view(-1, n_step) would raise)"
+        A = self.action_size
+        dev = self.device
+        st = getattr(self, "_st", None)
+        if st is None or st["NT"] != NT:
+            st = {"NT": NT,
+                  "out": torch.empty(NT, net.nout, device=dev),
+                  "value": torch.empty(NT, device=dev),
+                  "logp_old": torch.empty(NT, A if self.continuous else 1, device=dev),
+                  "adv": torch.empty(NT, device=dev), "ret": torch.empty(NT, device=dev),
+                  "next_value": torch.empty(NT, device=dev),
+                  "perm": torch.empty(NT, dtype=torch.int32, device=dev)}
+            self._st = st
+        st["state"] = state
+        st["action"] = action
+        mean_ret = self._advantages(st, state, action, reward, done, next_state, last_next_state, next_rows, N, T)
 
         # ---- optimisation epochs (ppo.py:114-175) ----
         B = self.batch_size

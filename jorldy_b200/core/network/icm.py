@@ -32,7 +32,48 @@ BN_EPS, BN_MOMENTUM = 1e-5, 0.1
 OBS_CLIP = 5.0
 
 
-class ICM_MLP(FlatNetwork):
+class BatchNormNetwork(FlatNetwork):
+    """A flat network with training-mode BatchNorm1d layers (csrc/icm.cu jb_bn_elu_fwd / _bwd, width HIDDEN): their
+    running buffers live in `self.buffers`, and state_dict puts each layer's buffers after its bias, in torch's module
+    order.  Shared by the ICM and the RND predictor."""
+
+    def state_dict(self):
+        out = OrderedDict()
+        for k, v in self.p.items():
+            out[k] = v.detach().clone()
+            if k.startswith("bn") and k.endswith(".bias"):
+                bn = k[:-len(".bias")]
+                for b in ("running_mean", "running_var", "num_batches_tracked"):
+                    out[f"{bn}.{b}"] = self.buffers[f"{bn}.{b}"].clone()
+        return out
+
+    def load_state_dict(self, sd):
+        sd = dict(sd)
+        bufs = {k: sd.pop(k) for k in list(sd) if k in self.buffers}
+        missing = [k for k in self.buffers if k not in bufs]
+        if missing:
+            raise KeyError(f"state_dict mismatch: missing {missing}")
+        super().load_state_dict(sd)
+        for k, v in bufs.items():
+            self.buffers[k].copy_(torch.as_tensor(v).to(self.buffers[k].dtype).reshape(self.buffers[k].shape))
+
+    def buffer_tensors(self):
+        return list(self.buffers.values())
+
+    def _bn_args(self, bn, M, tag):
+        if not self.batch_norm:
+            return [0] * 9
+        H = HIDDEN
+        b = self.buffers
+        return [ptr(self.p[f"{bn}.weight"]), ptr(self.p[f"{bn}.bias"]), ptr(b[f"{bn}.running_mean"]),
+                ptr(b[f"{bn}.running_var"]), ptr(b[f"{bn}.num_batches_tracked"]), BN_MOMENTUM, BN_EPS,
+                ptr(self._buf(tag + bn + ".mean", (H,))), ptr(self._buf(tag + bn + ".invstd", (H,)))]
+
+    def _partials(self, M, N, tag):
+        return self._buf(tag + "partials", (C.jb_col_partials_doubles(M, N),), torch.float64)
+
+
+class ICM_MLP(BatchNormNetwork):
     """`cnn` = True: D_in is the frame stack's [C, H, W] and the CNN trunk feeds fc1 (icm_cnn)."""
 
     def __init__(self, D_in, D_out, action_type, batch_norm=True, device=None, seed=None, cnn=False):
@@ -68,43 +109,6 @@ class ICM_MLP(FlatNetwork):
                 self.buffers[f"{bn}.running_mean"] = torch.zeros(H, device=self.device)
                 self.buffers[f"{bn}.running_var"] = torch.ones(H, device=self.device)
                 self.buffers[f"{bn}.num_batches_tracked"] = torch.zeros((), dtype=torch.int64, device=self.device)
-
-    # ---- state_dict with the BatchNorm buffers, in torch's module order ------------------------------------------------
-    def state_dict(self):
-        out = OrderedDict()
-        for k, v in self.p.items():
-            out[k] = v.detach().clone()
-            if k.startswith("bn") and k.endswith(".bias"):
-                bn = k[:-len(".bias")]
-                for b in ("running_mean", "running_var", "num_batches_tracked"):
-                    out[f"{bn}.{b}"] = self.buffers[f"{bn}.{b}"].clone()
-        return out
-
-    def load_state_dict(self, sd):
-        sd = dict(sd)
-        bufs = {k: sd.pop(k) for k in list(sd) if k in self.buffers}
-        missing = [k for k in self.buffers if k not in bufs]
-        if missing:
-            raise KeyError(f"state_dict mismatch: missing {missing}")
-        super().load_state_dict(sd)
-        for k, v in bufs.items():
-            self.buffers[k].copy_(torch.as_tensor(v).to(self.buffers[k].dtype).reshape(self.buffers[k].shape))
-
-    def buffer_tensors(self):
-        return list(self.buffers.values())
-
-    # ---- forward ---------------------------------------------------------------------------------------------------------
-    def _bn_args(self, bn, M, tag):
-        if not self.batch_norm:
-            return [0] * 9
-        H = HIDDEN
-        b = self.buffers
-        return [ptr(self.p[f"{bn}.weight"]), ptr(self.p[f"{bn}.bias"]), ptr(b[f"{bn}.running_mean"]),
-                ptr(b[f"{bn}.running_var"]), ptr(b[f"{bn}.num_batches_tracked"]), BN_MOMENTUM, BN_EPS,
-                ptr(self._buf(tag + bn + ".mean", (H,))), ptr(self._buf(tag + bn + ".invstd", (H,)))]
-
-    def _partials(self, M, N, tag):
-        return self._buf(tag + "partials", (C.jb_col_partials_doubles(M, N),), torch.float64)
 
     def _stacked_rows(self, s, s_next, idx, M, tag):
         """The CNN trunk's input: the rows idx of s, then those of s_next, as one row source of 2M stacks (frame

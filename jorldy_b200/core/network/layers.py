@@ -2,6 +2,7 @@
 from ..dev import C, ptr, stream_ptr
 
 
+import ctypes
 import os
 
 TC_MIN_ROWS = 1024     # below this a 128x128 tile grid cannot fill the 132 SMs: stay on the fp32 FFMA tiles
@@ -55,38 +56,26 @@ def linear_io_bwd_dw(dy, x, dw, db):
     C.jb_colsum(ptr(dy), M, out_f, ptr(db), 0, stream_ptr())
 
 
+def _ptrs(ts, kind=ctypes.c_void_p):
+    return (kind * len(ts))(*ts)
+
+
 def heads_fwd(h, heads, out):
-    """heads: list of up to 3 (w, b) pairs, w [n,H]."""
+    """heads: list of up to 4 (w, b) pairs, w [n,H]."""
     M, H = h.shape
-    a = []
-    for i in range(3):
-        if i < len(heads):
-            w, b = heads[i]
-            a += [ptr(w), ptr(b), w.shape[0]]
-        else:
-            a += [0, 0, 0]
-    C.jb_heads_fwd(ptr(h), M, H, *a, ptr(out), stream_ptr())
+    C.jb_heads_fwd_n(ptr(h), M, H, len(heads), _ptrs([ptr(w) for w, _ in heads]), _ptrs([ptr(b) for _, b in heads]),
+                     _ptrs([w.shape[0] for w, _ in heads], ctypes.c_int), ptr(out), stream_ptr())
 
 
 def heads_bwd_dx(dout, h, heads, dh):
     M, H = h.shape
-    a = []
-    for i in range(3):
-        if i < len(heads):
-            a += [ptr(heads[i][0]), heads[i][0].shape[0]]
-        else:
-            a += [0, 0]
-    C.jb_heads_bwd_dx(ptr(dout), ptr(h), M, H, *a, ptr(dh), stream_ptr())
+    C.jb_heads_bwd_dx_n(ptr(dout), ptr(h), M, H, len(heads), _ptrs([ptr(w) for w, _ in heads]),
+                        _ptrs([w.shape[0] for w, _ in heads], ctypes.c_int), ptr(dh), stream_ptr())
 
 
 def heads_bwd_dw(dout, h, grads):
-    """grads: list of up to 3 (dw, db) pairs."""
+    """grads: list of up to 4 (dw, db) pairs."""
     M, H = h.shape
-    a = []
-    for i in range(3):
-        if i < len(grads):
-            dw, db = grads[i]
-            a += [ptr(dw), ptr(db), dw.shape[0]]
-        else:
-            a += [0, 0, 0]
-    C.jb_heads_bwd_dw(ptr(dout), ptr(h), M, H, *a, stream_ptr())
+    C.jb_heads_bwd_dw_n(ptr(dout), ptr(h), M, H, len(grads), _ptrs([ptr(dw) for dw, _ in grads]),
+                        _ptrs([ptr(db) for _, db in grads]), _ptrs([dw.shape[0] for dw, _ in grads], ctypes.c_int),
+                        stream_ptr())

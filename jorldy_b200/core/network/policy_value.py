@@ -1,4 +1,4 @@
-"""Trunk + narrow-heads networks: head -> l (Linear+ReLU) -> up to three narrow output heads.
+"""Trunk + narrow-heads networks: head -> l (Linear+ReLU) -> up to four narrow output heads.
 
 Actor-critic (jorldy/core/network/policy_value.py:8-22 discrete, :38-57 continuous) and the plain
 Q network (q_network.py:8-20) share this shape.  forward_raw returns the PRE-activation head
@@ -101,3 +101,17 @@ class DiscretePolicyValue(_PolicyValue):
 class ContinuousPolicyValue(_PolicyValue):
     def _out_heads(self, D_out):
         return [("mu", D_out, "linear"), ("log_std", D_out, "tanh"), ("v", 1, "linear")]
+
+
+class DiscretePolicyTwoValue(_PolicyValue):
+    """RND-PPO's policy network: PPO's discrete heads and an intrinsic value head v_i, out = [pi | v | v_i]."""
+
+    def _out_heads(self, D_out):
+        return [("pi", D_out, "policy"), ("v", 1, "linear"), ("v_i", 1, "linear")]
+
+
+class ContinuousPolicyTwoValue(_PolicyValue):
+    """RND-PPO's policy network: PPO's continuous heads and v_i, out = [mu | log_std | v | v_i]."""
+
+    def _out_heads(self, D_out):
+        return [("mu", D_out, "linear"), ("log_std", D_out, "tanh"), ("v", 1, "linear"), ("v_i", 1, "linear")]

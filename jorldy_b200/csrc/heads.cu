@@ -167,16 +167,28 @@ heads_bwd_dw_kernel(const float* __restrict__ dout, const float* __restrict__ h,
   }
 }
 
-static bool fill_rows(HeadRows& hr, const float* const* w, const float* const* b, const int* n, int H) {
+constexpr int MAX_HEADS = 4;  // a continuous two-value policy: mu, log_std, v, v_i
+
+static bool fill_rows(HeadRows& hr, int n_heads, const float* const* w, const float* const* b, const int* n, int H) {
   int o = 0;
-  for (int g = 0; g < 3; ++g)
+  for (int g = 0; g < n_heads; ++g)
     for (int q = 0; q < n[g]; ++q, ++o) {
       if (o >= MAX_NOUT || !w[g]) return false;
       hr.w[o] = w[g] + (size_t)q * H;
-      hr.b[o] = b[g] ? b[g] + q : nullptr;
+      hr.b[o] = b && b[g] ? b[g] + q : nullptr;
     }
   for (; o < MAX_NOUT; ++o) { hr.w[o] = nullptr; hr.b[o] = nullptr; }
   return true;
+}
+
+static int total_outputs(int n_heads, const int* n) {
+  if (n_heads <= 0 || n_heads > MAX_HEADS || !n) return -1;
+  int nout = 0;
+  for (int g = 0; g < n_heads; ++g) {
+    if (n[g] < 0) return -1;
+    nout += n[g];
+  }
+  return nout > 0 && nout <= MAX_NOUT ? nout : -1;
 }
 
 }  // namespace
@@ -189,40 +201,36 @@ JB_API int jb_mlp_in_fwd(const float* x, const int32_t* idx, const float* w1, co
   return jb_check_launch();
 }
 
-// up to 3 heads; pass NULL/0 for unused ones.  out is [M, n0+n1+n2].
-JB_API int jb_heads_fwd(const float* h, int M, int H, const float* w0, const float* b0, int n0, const float* w1,
-                        const float* b1, int n1, const float* w2, const float* b2, int n2, float* out, void* stream) {
-  const int nout = n0 + n1 + n2;
-  if (!h || !out || M <= 0 || H <= 0 || nout <= 0 || nout > MAX_NOUT) return JB_ERR_INVALID;
-  const float* w[3] = {w0, w1, w2}; const float* b[3] = {b0, b1, b2}; const int n[3] = {n0, n1, n2};
-  for (int g = 0; g < 3; ++g) if (n[g] > 0 && (!w[g] || !b[g])) return JB_ERR_INVALID;
+JB_API int jb_heads_fwd_n(const float* h, int M, int H, int n_heads, const float* const* w, const float* const* b,
+                          const int* n, float* out, void* stream) {
+  const int nout = total_outputs(n_heads, n);
+  if (!h || !out || !w || !b || M <= 0 || H <= 0 || nout < 0) return JB_ERR_INVALID;
+  for (int g = 0; g < n_heads; ++g) if (n[g] > 0 && (!w[g] || !b[g])) return JB_ERR_INVALID;
   HeadRows hr;
-  if (!fill_rows(hr, w, b, n, H)) return JB_ERR_INVALID;
+  if (!fill_rows(hr, n_heads, w, b, n, H)) return JB_ERR_INVALID;
   const int threads = 256;
   heads_fwd_kernel<<<jb_div_up((long long)M * 32, threads), threads, 0, (cudaStream_t)stream>>>(h, M, H, hr, nout, out);
   return jb_check_launch();
 }
 
-JB_API int jb_heads_bwd_dx(const float* dout, const float* h, int M, int H, const float* w0, int n0, const float* w1,
-                           int n1, const float* w2, int n2, float* dh, void* stream) {
-  const int nout = n0 + n1 + n2;
-  if (!dout || !h || !dh || M <= 0 || H <= 0 || nout <= 0 || nout > MAX_NOUT) return JB_ERR_INVALID;
-  const float* w[3] = {w0, w1, w2}; const float* b[3] = {nullptr, nullptr, nullptr}; const int n[3] = {n0, n1, n2};
+JB_API int jb_heads_bwd_dx_n(const float* dout, const float* h, int M, int H, int n_heads, const float* const* w,
+                             const int* n, float* dh, void* stream) {
+  const int nout = total_outputs(n_heads, n);
+  if (!dout || !h || !dh || !w || M <= 0 || H <= 0 || nout < 0) return JB_ERR_INVALID;
   HeadRows hr;
-  if (!fill_rows(hr, w, b, n, H)) return JB_ERR_INVALID;
+  if (!fill_rows(hr, n_heads, w, nullptr, n, H)) return JB_ERR_INVALID;
   dim3 grid(jb_div_up(H, 128), M);
   heads_bwd_dx_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(dout, h, M, H, hr, nout, dh);
   return jb_check_launch();
 }
 
-JB_API int jb_heads_bwd_dw(const float* dout, const float* h, int M, int H, float* dw0, float* db0, int n0, float* dw1,
-                           float* db1, int n1, float* dw2, float* db2, int n2, void* stream) {
-  const int nout = n0 + n1 + n2;
-  if (!dout || !h || M <= 0 || H <= 0 || nout <= 0 || nout > MAX_NOUT) return JB_ERR_INVALID;
-  float* dw[3] = {dw0, dw1, dw2}; float* db[3] = {db0, db1, db2}; const int n[3] = {n0, n1, n2};
+JB_API int jb_heads_bwd_dw_n(const float* dout, const float* h, int M, int H, int n_heads, float* const* dw,
+                             float* const* db, const int* n, void* stream) {
+  const int nout = total_outputs(n_heads, n);
+  if (!dout || !h || !dw || !db || M <= 0 || H <= 0 || nout < 0) return JB_ERR_INVALID;
   HeadGradRows gr;
   int o = 0;
-  for (int g = 0; g < 3; ++g)
+  for (int g = 0; g < n_heads; ++g)
     for (int q = 0; q < n[g]; ++q, ++o) {
       if (!dw[g] || !db[g]) return JB_ERR_INVALID;
       gr.dw[o] = dw[g] + (size_t)q * H;
@@ -231,4 +239,23 @@ JB_API int jb_heads_bwd_dw(const float* dout, const float* h, int M, int H, floa
   for (; o < MAX_NOUT; ++o) { gr.dw[o] = nullptr; gr.db[o] = nullptr; }
   heads_bwd_dw_kernel<<<jb_div_up(H, 32), dim3(32, DW_ROWS), 0, (cudaStream_t)stream>>>(dout, h, M, H, gr, nout);
   return jb_check_launch();
+}
+
+// The three-head entry points: pass NULL/0 for unused heads.  out is [M, n0+n1+n2].
+JB_API int jb_heads_fwd(const float* h, int M, int H, const float* w0, const float* b0, int n0, const float* w1,
+                        const float* b1, int n1, const float* w2, const float* b2, int n2, float* out, void* stream) {
+  const float* w[3] = {w0, w1, w2}; const float* b[3] = {b0, b1, b2}; const int n[3] = {n0, n1, n2};
+  return jb_heads_fwd_n(h, M, H, 3, w, b, n, out, stream);
+}
+
+JB_API int jb_heads_bwd_dx(const float* dout, const float* h, int M, int H, const float* w0, int n0, const float* w1,
+                           int n1, const float* w2, int n2, float* dh, void* stream) {
+  const float* w[3] = {w0, w1, w2}; const int n[3] = {n0, n1, n2};
+  return jb_heads_bwd_dx_n(dout, h, M, H, 3, w, n, dh, stream);
+}
+
+JB_API int jb_heads_bwd_dw(const float* dout, const float* h, int M, int H, float* dw0, float* db0, int n0, float* dw1,
+                           float* db1, int n1, float* dw2, float* db2, int n2, void* stream) {
+  float* dw[3] = {dw0, dw1, dw2}; float* db[3] = {db0, db1, db2}; const int n[3] = {n0, n1, n2};
+  return jb_heads_bwd_dw_n(dout, h, M, H, 3, dw, db, n, stream);
 }

@@ -97,15 +97,7 @@ __global__ void ppo_prepass_discrete_kernel(const float* __restrict__ out, const
                                             float* __restrict__ logp_old) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
-  float lg[NA], lsm[NA];
-#pragma unroll
-  for (int a = 0; a < NA; ++a) lg[a] = a < A ? out[(size_t)m * nout + a] : 0.f;
-  log_softmax_row<NA>(lg, A, lsm);
-  const int a = action[m];
-  float la = 0.f;                              // lsm[a] without a run-time register index
-#pragma unroll
-  for (int q = 0; q < NA; ++q) if (q == a) la = lsm[q];
-  logp_old[m] = logf(expf(la));                // pi.gather(1, a).log(), pi = exp(log_softmax)
+  logp_old[m] = jbppo::logp_discrete<NA>(out + (size_t)m * nout, A, action[m]);
   value[m] = out[(size_t)m * nout + A];
 }
 
@@ -114,39 +106,11 @@ __global__ void ppo_prepass_continuous_kernel(const float* __restrict__ out, con
                                               float* __restrict__ logp_old /*[M,A]*/) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
-  const float log_sqrt_2pi = 0.9189385332046727f;
-  for (int a = 0; a < A; ++a) {
-    const float mu = fminf(fmaxf(out[(size_t)m * nout + a], -5.f), 5.f);
-    const float sd = expf(tanhf(out[(size_t)m * nout + A + a]));
-    const float z = atanh_clamped(action[(size_t)m * A + a]);
-    const float d = z - mu;
-    logp_old[(size_t)m * A + a] = -(d * d) / (2.f * (sd * sd)) - logf(sd) - log_sqrt_2pi;
-  }
+  jbppo::logp_continuous(out + (size_t)m * nout, A, action + (size_t)m * A, logp_old + (size_t)m * A);
   value[m] = out[(size_t)m * nout + 2 * A];
 }
 
 // ---- loss -------------------------------------------------------------------------------------
-// fixed-order block reduction; result broadcast to all threads
-template <int NV>
-__device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float x = v[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
-    if (lane == 0) smem[q * 32 + warp] = x;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float t = 0.f;
-    for (int w = 0; w < nw; ++w) t += smem[q * 32 + w];
-    v[q] = t;
-  }
-  __syncthreads();
-}
-
 // NA: compile-time bound on A, see jbppo::row.  The 18-wide row holds ~145 live registers: min-blocks 1 lets ptxas use
 // them instead of spilling at its default 128 (0 leaves the 8-wide instantiations unconstrained, as before).
 template <bool CONT, int NA>
@@ -167,7 +131,7 @@ ppo_loss_kernel(const float* __restrict__ out, const int32_t* __restrict__ idx, 
     const float d1 = v - ret, d2 = vclip - ret;
     c[0] += d1 * d1; c[1] += d2 * d2;
   }
-  block_sum<2>(c, sred);
+  jbppo::block_sum<2>(c, sred);
   const float c1 = c[0] * invB, c2 = c[1] * invB;
   float w1, w2;
   jbppo::critic_weights(c1, c2, w1, w2);
@@ -192,7 +156,7 @@ ppo_loss_kernel(const float* __restrict__ out, const int32_t* __restrict__ idx, 
     st[0] = ro.surr_min; st[1] = ro.ent;
     max_ratio = ro.ratio; min_prob = ro.pmin;
   }
-  block_sum<2>(st, sred);
+  jbppo::block_sum<2>(st, sred);
   float mr = jb_warp_max(max_ratio), mp = jb_warp_min(min_prob);
   __shared__ float smax[32], smin_[32];
   if ((threadIdx.x & 31) == 0) { smax[threadIdx.x >> 5] = mr; smin_[threadIdx.x >> 5] = mp; }
@@ -212,19 +176,7 @@ ppo_loss_kernel(const float* __restrict__ out, const int32_t* __restrict__ idx, 
 __global__ void ppo_stats_finalize_kernel(float* __restrict__ stats, int n_cta, int B, int A, int cont,
                                           float* __restrict__ acc) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  float s0 = 0.f, s1 = 0.f, mr = -INFINITY, mp = INFINITY;
-  for (int k = 0; k < n_cta; ++k) {
-    const float* sp = stats + 8 + 4 * k;
-    s0 += sp[0]; s1 += sp[1]; mr = fmaxf(mr, sp[2]); mp = fminf(mp, sp[3]);
-  }
-  const float invB = 1.0f / (float)B;
-  stats[0] = -s0 * invB;                                   // actor_loss
-  stats[2] = -s1 * invB / (cont ? (float)A : 1.f);         // entropy_loss
-  stats[3] = mr; stats[4] = mp;
-  if (acc) {
-    acc[0] += stats[0]; acc[1] += stats[1]; acc[2] += stats[2];
-    acc[3] = fmaxf(acc[3], mr); acc[4] = fminf(acc[4], mp); acc[5] += 1.f;
-  }
+  jbppo::fold_stats(stats, n_cta, B, A, cont, acc);
 }
 
 // cur_idx[0..B) = perm[cursor*B .. cursor*B+B); cursor += 1.  Lets a captured CUDA graph of one

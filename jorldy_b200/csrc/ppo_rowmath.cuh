@@ -201,4 +201,70 @@ __device__ __forceinline__ void critic_weights(float c1, float c2, float& w1, fl
   w2 = 1.f - w1;
 }
 
+// log_prob_old of one pre-pass row (ppo.py:83-93), shared by PPO's and RND-PPO's pre-pass kernels.
+// Discrete: pi.gather(1, a).log() with pi = exp(log_softmax(o[0..A))).  NA: compile-time bound on A.
+template <int NA>
+__device__ __forceinline__ float logp_discrete(const float* o, int A, int a) {
+  float lg[NA], lsm[NA];
+#pragma unroll
+  for (int q = 0; q < NA; ++q) lg[q] = q < A ? o[q] : 0.f;
+  log_softmax_row<NA>(lg, A, lsm);
+  float la = 0.f;                              // lsm[a] without a run-time register index
+#pragma unroll
+  for (int q = 0; q < NA; ++q) if (q == a) la = lsm[q];
+  return logf(expf(la));
+}
+
+// Continuous: lp[a] = Normal(clamp(mu, +-5), exp(tanh(log_std))).log_prob(atanh(clamp(action[a], +-(1 - 1e-7)))).
+__device__ __forceinline__ void logp_continuous(const float* o, int A, const float* action, float* lp) {
+  const float log_sqrt_2pi = 0.9189385332046727f;
+  for (int a = 0; a < A; ++a) {
+    const float mu = fminf(fmaxf(o[a], -5.f), 5.f);
+    const float sd = expf(tanhf(o[A + a]));
+    const float z = atanh_clamped(action[a]);
+    const float d = z - mu;
+    lp[a] = -(d * d) / (2.f * (sd * sd)) - logf(sd) - log_sqrt_2pi;
+  }
+}
+
+// fixed-order block reduction of NV values; result broadcast to all threads
+template <int NV>
+__device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+#pragma unroll
+  for (int q = 0; q < NV; ++q) {
+    float x = v[q];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+    if (lane == 0) smem[q * 32 + warp] = x;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int q = 0; q < NV; ++q) {
+    float t = 0.f;
+    for (int w = 0; w < nw; ++w) t += smem[q * 32 + w];
+    v[q] = t;
+  }
+  __syncthreads();
+}
+
+// One thread folds the per-CTA partials (stats + 8 + 4 k: surr_min sum, entropy sum, max ratio, min prob) in CTA order
+// into stats[0] actor_loss, stats[2] entropy_loss, stats[3] max_ratio, stats[4] min_prob; stats[1] (the critic loss) is
+// the loss kernel's.  acc (may be NULL): acc[0..2] += stats[0..2], acc[3] = max, acc[4] = min, acc[5] += 1.
+__device__ __forceinline__ void fold_stats(float* stats, int n_cta, int B, int A, int cont, float* acc) {
+  float s0 = 0.f, s1 = 0.f, mr = -INFINITY, mp = INFINITY;
+  for (int k = 0; k < n_cta; ++k) {
+    const float* sp = stats + 8 + 4 * k;
+    s0 += sp[0]; s1 += sp[1]; mr = fmaxf(mr, sp[2]); mp = fminf(mp, sp[3]);
+  }
+  const float invB = 1.0f / (float)B;
+  stats[0] = -s0 * invB;                                   // actor_loss
+  stats[2] = -s1 * invB / (cont ? (float)A : 1.f);         // entropy_loss
+  stats[3] = mr; stats[4] = mp;
+  if (acc) {
+    acc[0] += stats[0]; acc[1] += stats[1]; acc[2] += stats[2];
+    acc[3] = fmaxf(acc[3], mr); acc[4] = fminf(acc[4], mp); acc[5] += 1.f;
+  }
+}
+
 }  // namespace jbppo
