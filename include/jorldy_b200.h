@@ -260,6 +260,40 @@ JB_API int jb_adv_mix(const float* adv_e, const float* adv_i, int N, int T, floa
                       int standardize, float* adv, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * REINFORCE (Williams, 1992) on whole episodes, csrc/reinforce.cu.  The episode ring keeps every unlearned step of N envs:
+ * reward / done [N, L] f32, action int64 [N, L] (discrete) or f32 [N, L, A] (continuous); step t of every env lives in
+ * column t mod L.  pos (device int64) counts the steps written; head[e] (device int64 [N]) is env e's oldest unlearned
+ * step.  No atomics: every entry point is bit-reproducible.
+ *   jb_episode_returns  for each env, the completed steps [head[e], last done in [head[e], pos)]: per episode the
+ *                       discounted returns G_t = r_t + gamma G_{t+1} (G = r at the episode's done) in float64, with
+ *                       `standardize` (G - mean) / (std + 1e-7) with the episode's own mean and ddof-0 std; written as
+ *                       fp32 into ret_ring [N, L] at the steps' columns.  count[e] = the completed steps; head[e] moves
+ *                       past them.
+ *   jb_episode_rows     offsets [N] (workspace) = exclusive scan of count in env order; M (device int) = the total;
+ *                       idx [.] = e L + column and ret [.] of every completed step, env-major and oldest first, padded
+ *                       with idx 0 / ret 0 to a multiple of C.  idx / ret hold at least ceil(N L / C) C entries.
+ *                       N L + C must fit an int32.
+ *   jb_reinforce_loss   one chunk of C rows: chunk k = *cursor - 1 (after jb_take_minibatch; cursor NULL: chunk 0)
+ *                       covers idx / ret entries [k C, k C + C); out [C, nout] holds the head outputs of those ring rows
+ *                       (discrete logits, nout = A <= 18; continuous raw [mu | log_std], nout = 2A, A <= 8).
+ *                       dout [C, nout] = d loss / d out of loss = -(1/M) sum log pi(a) ret (continuous: -(1/(M A)) sum
+ *                       over rows and dims, mu = clamp(raw, +-5), std = exp(tanh(raw)), z = atanh(clamp(a, +-(1-1e-7)))).
+ *                       Entries at or past the device M are padding: dout rows 0, no loss.  partials holds
+ *                       jb_reinforce_loss_partials(C) floats, folded in CTA order: acc[0] += the chunk's share of the
+ *                       loss, acc[1] += 1.  A device M <= 0 adds nothing.
+ *   jb_add_f32          y += x over n floats (chunk gradients summed in chunk order).
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_episode_returns(const float* reward, const float* done, int N, int L, const long long* pos, long long* head,
+                              double gamma, int standardize, float* ret_ring, int* count, void* stream);
+JB_API int jb_episode_rows(const int* count, const long long* head, const float* ret_ring, int N, int L, int C,
+                           int* offsets, int32_t* idx, float* ret, int* M, void* stream);
+JB_API int jb_reinforce_loss_partials(int C);
+JB_API int jb_reinforce_loss(int continuous, const float* out, const int32_t* rows, const float* ret,
+                             const long long* cursor, const int* M, int C, const void* action, int A, int nout,
+                             float* dout, float* partials, float* acc, void* stream);
+JB_API int jb_add_f32(float* y, const float* x, long long n, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * ICM-PPO (Pathak et al., ICML 2017) on the PPO rollout path, csrc/icm.cu.  Column reductions split the rows into
  * chunks of 256 and fold the chunks' float64 partial sums in chunk order; `partials` holds jb_col_partials_doubles(M, N)
  * doubles.  No atomics anywhere: every entry point is bit-reproducible.

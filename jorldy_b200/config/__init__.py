@@ -8,7 +8,8 @@ pendulum / atari(synthetic) / mujoco(synthetic dims), plus the discrete-action S
 which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the V-MPO
 paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys,
 `config.rnd_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the RND keys,
-and `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows; an existing JORLDY config directory on sys.path takes precedence
+`config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows, and
+`config.reinforce.{cartpole,mountaincar,pendulum,mujoco}`, PPO's rows with the REINFORCE keys; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -192,6 +193,20 @@ def _rnd_ppo_config(env):
     return d
 
 
+# REINFORCE: PPO's env, optimiser and train rows for the same env without distributed_batch_size (REINFORCE has no
+# minibatch), and PPO's network with the value head dropped.  These are this project's choices; a JORLDY config
+# directory on sys.path takes precedence.
+_REINFORCE_ENVS = ("cartpole", "mountaincar", "pendulum", "mujoco")
+
+
+def _reinforce_config(env):
+    d = _ppo_config(env)
+    d["train"].pop("distributed_batch_size", None)
+    d["agent"] = dict(name="reinforce", network=d["agent"]["network"][:-len("_value")], gamma=0.99,
+                      use_standardization=True, lr_decay=True)
+    return d
+
+
 # ---- continuous off-policy family: jorldy/config/{ddpg,td3,sac}/{cartpole,pendulum,mujoco}.py --------------------------------
 _TRAIN_MUJOCO = dict(training=True, load_path=None, run_step=1000000, print_period=10000, save_period=100000, eval_iteration=10)
 _AC_ENVS = {"ddpg": ("cartpole", "pendulum", "mujoco"), "td3": ("cartpole", "mujoco"), "sac": ("cartpole", "pendulum", "mujoco")}
@@ -295,6 +310,7 @@ def available():
     out += [f"config.icm_ppo.{e}" for e in _ICM_PPO_ENVS]
     out += [f"config.rnd_ppo.{e}" for e in _RND_PPO_ENVS]
     out += [f"config.mpo.{e}" for e in _MPO_ENVS]
+    out += [f"config.reinforce.{e}" for e in _REINFORCE_ENVS]
     return out
 
 
@@ -319,6 +335,8 @@ def load(config_path):
         d = _rnd_ppo_config(env)
     elif agent == "mpo" and env in _MPO_ENVS:
         d = _mpo_config(env)
+    elif agent == "reinforce" and env in _REINFORCE_ENVS:
+        d = _reinforce_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
     elif agent == "sac_discrete" and env in ("cartpole", "atari"):

@@ -12,10 +12,11 @@ from .vmpo import VMPO
 from .icm_ppo import ICM_PPO
 from .mpo import MPO
 from .rnd_ppo import RND_PPO
+from .reinforce import REINFORCE
 
 agent_dict = OrderedDict(sorted(dict(ape_x=ApeX, c51=C51, ddpg=DDPG, double=Double, dqn=DQN, dueling=Dueling, icm_ppo=ICM_PPO, iqn=IQN,
                                      m_dqn=MDQN, m_iqn=MIQN, mpo=MPO, multistep=Multistep, noisy=Noisy, per=PER, ppo=PPO, qrdqn=QRDQN, r2d2=R2D2,
-                                     rainbow=Rainbow, rainbow_iqn=RainbowIQN, rnd_ppo=RND_PPO, sac=SAC, td3=TD3,
+                                     rainbow=Rainbow, rainbow_iqn=RainbowIQN, reinforce=REINFORCE, rnd_ppo=RND_PPO, sac=SAC, td3=TD3,
                                      vmpo=VMPO).items()))
 
 

@@ -5,7 +5,8 @@
 `DeviceRollout` is the HBM-resident [N, T, ...] structure-of-arrays the batched collect kernels
 write straight into (no host hop): actor-major like the reference's concatenation order
 (distributed_manager.py:30), so GAE's `view(-1, n_step)` rows are envs.  `FrameRollout` is its variant for
-Atari-shaped frame stacks, with states kept as single-frame references (buffer/frame_store.py).
+Atari-shaped frame stacks, with states kept as single-frame references (buffer/frame_store.py).  `EpisodeRing` keeps
+every unlearned step of N envs across rounds, for learners that need whole episodes (REINFORCE).
 """
 import numpy as np
 import torch
@@ -104,6 +105,53 @@ class DeviceRollout:
 
     def clear(self):
         self.t = 0
+
+
+class EpisodeRing:
+    """Every unlearned step of N envs, for learners that need whole episodes (REINFORCE): state [N, L, D], action
+    ([N, L] int64 / [N, L, A] f32), reward and done [N, L].  All envs step in lockstep, so step t of every env lives in
+    column t mod L.  `pos` (device int64) counts the steps written and advances on the device, so one captured collect
+    graph serves every round; head [N] (device int64) is each env's oldest unlearned step, which the learner moves past
+    the episodes it consumes (jb_episode_returns).
+
+    Capacity: after a learn, an env's only unlearned steps are its unfinished episode, at most max_steps - 1 steps under
+    the env's time limit; a round adds T_round more.  So L = max_steps - 1 + T_round (`capacity`) never overwrites an
+    unlearned step."""
+
+    def __init__(self, num_envs, capacity, state_size, action_size, action_type, device=None):
+        dev = require_cuda(device)
+        N, L = num_envs, capacity
+        self.N, self.L, self.device = N, L, dev
+        self.state = torch.zeros(N, L, state_size, dtype=torch.float32, device=dev)
+        if action_type == "discrete":
+            self.action = torch.zeros(N, L, dtype=torch.int64, device=dev)
+        else:
+            self.action = torch.zeros(N, L, action_size, dtype=torch.float32, device=dev)
+        self.reward = torch.zeros(N, L, dtype=torch.float32, device=dev)
+        self.done = torch.zeros(N, L, dtype=torch.float32, device=dev)
+        self.pos = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.head = torch.zeros(N, dtype=torch.int64, device=dev)
+        self._col = torch.zeros(1, dtype=torch.int64, device=dev)     # pos mod L, the column being written
+
+    @staticmethod
+    def capacity(max_steps, n_round):
+        return int(max_steps) - 1 + int(n_round)
+
+    def write_state(self, state):
+        """First half of a transition: the state acted on, into column pos mod L."""
+        torch.remainder(self.pos, self.L, out=self._col)
+        self.state.index_copy_(1, self._col, state.view(self.N, 1, -1))
+
+    def write_after_step(self, action, reward, done, next_state=None):
+        """Second half of a transition (write_state() already stored its state); advances pos.  next_state is unused:
+        REINFORCE never bootstraps."""
+        if self.action.dim() == 2:
+            self.action.index_copy_(1, self._col, action.view(self.N, 1).to(torch.int64))
+        else:
+            self.action.index_copy_(1, self._col, action.view(self.N, 1, -1))
+        self.reward.index_copy_(1, self._col, reward.view(self.N, 1))
+        self.done.index_copy_(1, self._col, done.view(self.N, 1))
+        self.pos.add_(1)
 
 
 class FrameRollout(DeviceRollout):

@@ -7,7 +7,7 @@ randomness).
 """
 import torch
 
-from .buffer import DeviceRollout, FrameRollout, frame_store
+from .buffer import DeviceRollout, EpisodeRing, FrameRollout, frame_store
 
 
 class RolloutCollector:
@@ -64,6 +64,57 @@ class RolloutCollector:
         self._graph.replay()
         self.rollout.t = self.T
         return self.rollout
+
+
+class EpisodeCollector:
+    """Whole-episode collection for REINFORCE: a round is n_round steps of act -> env.step_device -> ring write for
+    every env, captured in ONE CUDA graph like RolloutCollector's (the ring's write column advances on the device);
+    use_cuda_graph=False runs the same launches eagerly.  The ring holds L = env.max_steps - 1 + n_round steps per env
+    (EpisodeRing), so an env needs a time limit."""
+
+    def __init__(self, env, agent, n_round, use_cuda_graph=True):
+        if getattr(env, "frame_stack", False):
+            raise NotImplementedError("episode rings of frame stacks are not implemented: an episode can outlive any "
+                                      "frame store that fits on the device")
+        max_steps = getattr(env, "max_steps", None)
+        if not max_steps:
+            raise ValueError(f"{type(env).__name__} has no max_steps time limit: an unfinished episode could outgrow "
+                             "any episode ring")
+        self.env, self.agent, self.T = env, agent, int(n_round)
+        self.ring = EpisodeRing(env.num_envs, EpisodeRing.capacity(max_steps, self.T), env.state_size, env.action_size,
+                                env.action_type, device=agent.device)
+        self.use_cuda_graph = use_cuda_graph
+        self._graph = None
+        env.reset_device()
+
+    def _collect_eager(self):
+        env, agent, ring = self.env, self.agent, self.ring
+        for _ in range(self.T):
+            ring.write_state(env.obs)
+            action = agent.act_device(env.obs, training=True)
+            next_obs, reward, done = env.step_device(action)
+            ring.write_after_step(action, reward, done)
+
+    def collect(self):
+        """Appends n_round steps of every env to self.ring; returns it."""
+        if not self.use_cuda_graph:
+            self._collect_eager()
+            return self.ring
+        if self._graph is None:
+            # warm-up on a side stream (allocates workspaces; its steps are real ones), then capture the round
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._collect_eager()
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._collect_eager()
+            self._graph = g
+            return self.ring
+        self._graph.replay()
+        return self.ring
 
 
 class NStepAssembler:

@@ -215,15 +215,20 @@ __device__ __forceinline__ float logp_discrete(const float* o, int A, int a) {
   return logf(expf(la));
 }
 
+// Normal(mu, sd).log_prob(z) of one action dimension.
+__device__ __forceinline__ float normal_logpdf(float z, float mu, float sd) {
+  const float log_sqrt_2pi = 0.9189385332046727f;
+  const float d = z - mu;
+  return -(d * d) / (2.f * (sd * sd)) - logf(sd) - log_sqrt_2pi;
+}
+
 // Continuous: lp[a] = Normal(clamp(mu, +-5), exp(tanh(log_std))).log_prob(atanh(clamp(action[a], +-(1 - 1e-7)))).
 __device__ __forceinline__ void logp_continuous(const float* o, int A, const float* action, float* lp) {
-  const float log_sqrt_2pi = 0.9189385332046727f;
   for (int a = 0; a < A; ++a) {
     const float mu = fminf(fmaxf(o[a], -5.f), 5.f);
     const float sd = expf(tanhf(o[A + a]));
     const float z = atanh_clamped(action[a]);
-    const float d = z - mu;
-    lp[a] = -(d * d) / (2.f * (sd * sd)) - logf(sd) - log_sqrt_2pi;
+    lp[a] = normal_logpdf(z, mu, sd);
   }
 }
 

@@ -6,7 +6,8 @@ single_train            the reference's own per-step loop (run_mode.py:68-91) ov
 sync_distributed_train  the GPU-resident pipeline that replaces ray actors + the sync gather
                         (run_mode.py:163-198, manager/distributed_manager.py): `train.num_workers` becomes the
                         number of batched env instances stepped by one kernel; on-policy agents use
-                        RolloutCollector (+ learn_rollout), replay agents use ReplayCollector.  Under torchrun
+                        RolloutCollector (+ learn_rollout), REINFORCE EpisodeCollector (+ learn_episodes),
+                        replay agents use ReplayCollector.  Under torchrun
                         every rank runs this loop on its own GPU with gradient all-reduce (core/parallel.py).
 async_distributed_train same pipeline (there is no separate interact process to be asynchronous with:
                         collection and learning share the device; Ape-X per-actor epsilons are per env row).
@@ -20,7 +21,7 @@ import numpy as np
 import torch
 
 from .core import Agent, Env
-from .core.collect import ReplayCollector, RolloutCollector
+from .core.collect import EpisodeCollector, ReplayCollector, RolloutCollector
 from .manager import ConfigManager, LogManager, MetricManager
 
 
@@ -111,14 +112,23 @@ def sync_distributed_train(config_path, unknown):
         config_manager.dump(logger.path)
         metrics = MetricManager()
     on_policy = hasattr(agent, "learn_rollout")
+    episodic = hasattr(agent, "learn_episodes")        # REINFORCE: whole episodes from an episode ring
     update_period = int(config.train.update_period or getattr(agent, "n_step", 1))
-    collector = RolloutCollector(env, agent) if on_policy else ReplayCollector(env, agent, update_period)
+    if episodic:
+        collector = EpisodeCollector(env, agent, update_period)
+    else:
+        collector = RolloutCollector(env, agent) if on_policy else ReplayCollector(env, agent, update_period)
     step, t0 = 0, time.time()
     next_print = config.train.print_period
     next_save = config.train.save_period
     try:
         while step < config.train.run_step:
-            if on_policy:
+            if episodic:
+                result = agent.learn_episodes(collector.collect())
+                step += collector.T
+                if result and agent.lr_decay:            # a round that completed no episode learns nothing
+                    agent.learning_rate_decay(step)
+            elif on_policy:
                 result = agent.learn_rollout(collector.collect())
                 step += agent.n_step
                 if agent.lr_decay:
