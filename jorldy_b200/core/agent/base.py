@@ -7,6 +7,9 @@ import numpy as np
 import torch
 
 from ..dev import f32
+from ..network.base import FlatNetwork
+
+MULTIPLIERS = ("eta", "alpha_mu", "alpha_sigma")       # V-MPO's and MPO's learned multipliers, in their vector's order
 
 
 def cpu_state_dict(net):
@@ -22,6 +25,84 @@ def cpu_optimizer_state(optimizer):
             if torch.is_tensor(v):
                 st[k] = v.cpu()
     return sd
+
+
+class _Scalar(FlatNetwork):
+    """Learnable scalars held like a network so that the flat Adam applies: SAC's log_alpha (sac.py:95-100), or V-MPO's
+    [eta, alpha_mu, alpha_sigma] as one contiguous vector when `value` is a sequence."""
+
+    def __init__(self, name, value, device):
+        super().__init__(device)
+        values = [float(v) for v in np.atleast_1d(value)]
+        self._specs = [(name, (len(values),))]
+        self._allocate()
+        self.flat[:len(values)] = torch.tensor(values, dtype=torch.float32)
+
+
+# Adam is per element and the two parameter sets are disjoint, so the policy network's Adam and the curiosity network's
+# Adam are one torch Adam over network.parameters() + the curiosity network's parameters: the checkpoint stores that one
+# layout, the second optimiser's entries at the parameter indices after the network's.  ICM-PPO's and RND-PPO's
+# checkpoints share it.
+def two_adam_state(optimizer, aux_optimizer):
+    sd = cpu_optimizer_state(optimizer)
+    asd = cpu_optimizer_state(aux_optimizer)
+    P = len(optimizer.network.p)
+    for i, e in asd["state"].items():
+        sd["state"][P + i] = e
+    sd["param_groups"][0]["params"] = list(range(P + len(aux_optimizer.network.p)))
+    return sd
+
+
+def load_two_adam_state(sd, optimizer, aux_optimizer):
+    P, Q = len(optimizer.network.p), len(aux_optimizer.network.p)
+    st = sd.get("state", {})
+    get = lambda i: st[i] if i in st else st.get(str(i))
+    group = dict(sd["param_groups"][0])
+    optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {},
+                               "param_groups": [dict(group, params=list(range(P)))]})
+    aux_optimizer.load_state_dict({"state": {i: get(P + i) for i in range(Q)} if get(P) is not None else {},
+                                   "param_groups": [dict(group, params=list(range(Q)))]})
+
+
+# One torch-Adam layout over network.parameters() + [eta, alpha_mu, alpha_sigma]: the multipliers are the three parameter
+# indices after the network's, each a 0-d tensor; their values are stored under their own names too.  V-MPO's and MPO's
+# checkpoints share it.
+def joint_optimizer_state(optimizer, mult_optimizer):
+    sd = cpu_optimizer_state(optimizer)
+    P = len(optimizer.network.p)
+    step = float(mult_optimizer._step_dev.item())
+    if step > 0:
+        m, v = mult_optimizer.exp_avg[:3].cpu(), mult_optimizer.exp_avg_sq[:3].cpu()
+        for k in range(3):
+            sd["state"][P + k] = {"step": torch.tensor(step), "exp_avg": m[k].clone(), "exp_avg_sq": v[k].clone()}
+    sd["param_groups"][0]["params"] = list(range(P + 3))
+    return sd
+
+
+def multiplier_values(mult):
+    vals = mult.flat[:3].cpu()
+    return {name: vals[k].clone() for k, name in enumerate(MULTIPLIERS)}
+
+
+def load_joint_optimizer_state(sd, optimizer, mult_optimizer):
+    P = len(optimizer.network.p)
+    st = sd.get("state", {})
+    get = lambda i: st[i] if i in st else st.get(str(i))
+    group = dict(sd["param_groups"][0], params=list(range(P)))
+    optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {}, "param_groups": [group]})
+    mult_optimizer.param_groups[0]["lr"] = float(group["lr"])
+    if get(P) is not None:
+        for k in range(3):
+            e = get(P + k)
+            mult_optimizer.exp_avg[k].copy_(torch.as_tensor(e["exp_avg"]).reshape(()))
+            mult_optimizer.exp_avg_sq[k].copy_(torch.as_tensor(e["exp_avg_sq"]).reshape(()))
+        mult_optimizer._step_dev.fill_(int(float(get(P)["step"])))
+
+
+def load_multipliers(ck, mult):
+    for k, name in enumerate(MULTIPLIERS):
+        if name in ck:
+            mult.flat[k].copy_(torch.as_tensor(ck[name], dtype=torch.float32).reshape(()))
 
 
 class BaseAgent(ABC):
@@ -74,6 +155,10 @@ class BaseAgent(ABC):
     def interact_callback(self, transition):
         return transition
 
+    def _optimizers(self):
+        """Every optimiser a learn steps: learning_rate_decay's default list."""
+        return [self.optimizer]
+
     def learning_rate_decay(self, step, optimizers=None, mode="cosine"):
         """lr = lr0 * w(step/run_step) after every learn (base.py:93-111)."""
         frac = step / self.run_step
@@ -86,7 +171,7 @@ class BaseAgent(ABC):
         else:
             raise Exception(f"check learning rate decay mode again! => {mode}")
         if optimizers is None:
-            optimizers = [self.optimizer]
+            optimizers = self._optimizers()
         if not isinstance(optimizers, list):
             optimizers = [optimizers]
         for optimizer in optimizers:

@@ -16,26 +16,15 @@ import torch
 from ..buffer import ReplayBuffer
 from ..dev import C, ptr, require_cuda, stream_ptr
 from ..network import Network
-from ..network.base import FlatNetwork
 from ..optimizer import Optimizer
-from .base import BaseAgent, cpu_optimizer_state, cpu_state_dict
+from .base import BaseAgent, _Scalar, cpu_optimizer_state, cpu_state_dict
 
 _DEFAULT_OPTIM = {"actor": "adam", "critic": "adam", "actor_lr": 5e-4, "critic_lr": 1e-3}
 
 
-class _Scalar(FlatNetwork):
-    """Learnable scalars held like a network so that the flat Adam applies: SAC's log_alpha (sac.py:95-100), or V-MPO's
-    [eta, alpha_mu, alpha_sigma] as one contiguous vector when `value` is a sequence."""
-
-    def __init__(self, name, value, device):
-        super().__init__(device)
-        values = [float(v) for v in np.atleast_1d(value)]
-        self._specs = [(name, (len(values),))]
-        self._allocate()
-        self.flat[:len(values)] = torch.tensor(values, dtype=torch.float32)
-
-
 class _ActorCritic(BaseAgent):
+    replicas_only = True          # parallel.attach: several networks and optimisers per agent, no gradient exchange built
+    FAMILY = "the actor-critic family"
     action_type = "continuous"
     _n_critics = 1
     _strict_gate = False        # learn once memory.size > batch_size (SAC) instead of >= batch_size (DDPG, TD3)
@@ -169,7 +158,7 @@ class _ActorCritic(BaseAgent):
         if filled and step >= self.start_train_step:
             result = self.learn()
             if self.lr_decay:
-                self.learning_rate_decay(step, self._optimizers())
+                self.learning_rate_decay(step)
         if self._soft_in_process and self.num_learn > 0:
             self.update_target_soft()
         return result

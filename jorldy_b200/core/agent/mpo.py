@@ -27,18 +27,17 @@ import torch
 
 from ..dev import C, ptr, stream_ptr
 from ..optimizer import Optimizer
-from .base import cpu_optimizer_state, cpu_state_dict
-from .ddpg import _ActorCritic, _Scalar
-from .vmpo import joint_optimizer_state, load_joint_optimizer_state, load_multipliers, multiplier_values
+from .base import (_Scalar, cpu_optimizer_state, cpu_state_dict, joint_optimizer_state, load_joint_optimizer_state,
+                   load_multipliers, multiplier_values)
+from .ddpg import _ActorCritic
+from .ppo import MAX_ACTION_SIZE
 
 _PAIRS = {"discrete_policy": "discrete_q_network", "continuous_policy": "continuous_q_network"}
 _CRITIC_LOSS = {"retrace": 1, "1step_TD": 0}
-_MAX_A = {"discrete": 18, "continuous": 8}
 _SAMPLE_PURPOSE = 4          # Philox purpose id of the E-step normals (1: act, 2 / 3: the SAC / TD3 learn draws)
 
 
 class MPO(_ActorCritic):
-    replicas_only = True          # parallel.attach: no data-parallel learner for MPO
     FAMILY = "MPO"
     trajectory_windows = True     # ReplayCollector: store whole n-step windows with log mu
     _soft_in_process = False      # hard target copies inside learn()
@@ -65,8 +64,9 @@ class MPO(_ActorCritic):
             raise ValueError(f"num_sample {num_sample}: continuous MPO takes 1 <= num_sample <= 64")
         if not isinstance(state_size, int):
             raise ValueError("MPO takes an integer state_size (mlp head)")
-        if not 1 <= int(action_size) <= _MAX_A[self.action_type]:
-            raise ValueError(f"action_size {action_size}: {self.action_type} MPO takes at most {_MAX_A[self.action_type]} actions")
+        if not 1 <= int(action_size) <= MAX_ACTION_SIZE[self.action_type]:
+            raise ValueError(f"action_size {action_size}: {self.action_type} MPO takes at most "
+                             f"{MAX_ACTION_SIZE[self.action_type]} actions")
         opt = dict(optim_config)
         name, lr = opt.pop("name"), opt.pop("lr")
         self._common(state_size, action_size, hidden_size, actor, critic, head,

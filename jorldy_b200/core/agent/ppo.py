@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from ..buffer import FrameRollout, RolloutBuffer
-from ..dev import C, ptr, require_cuda, stream_ptr
+from ..dev import C, capture_after_warmup, ptr, require_cuda, stream_ptr
 from ..network import Network
 from ..optimizer import Optimizer
 from .base import BaseAgent
@@ -131,30 +131,45 @@ class PPO(BaseAgent):
 
     # ----------------------------------------------------------------------------------- learn --
     def _minibatch_step(self, st, idx, B):
-        """forward -> fused loss fwd/bwd -> backward -> (all-reduce) -> clip + Adam, for rollout rows idx[B]."""
+        """forward -> loss -> backward -> (all-reduce) -> clip + Adam, then _after_step, for rollout rows idx[B]."""
         net = self.network
         tag = f"mb{B}."
         out = net.forward_raw(st["state"], idx, B, tag=tag)
         dout = net._buf(tag + "dout", (B, net.nout))
-        stats = net._buf(tag + "stats", (8 + 4 * ((B + 255) // 256),))
-        C.jb_ppo_loss(int(self.continuous), ptr(out), ptr(idx), ptr(st["action"]), ptr(st["adv"]), ptr(st["ret"]),
-                      ptr(st["value"]), ptr(st["logp_old"]), B, self.action_size, net.nout, self.epsilon_clip,
-                      self.vf_coef, self.ent_coef, ptr(dout), ptr(stats), ptr(self._acc), stream_ptr())
+        self._loss(st, idx, B, out, dout, tag)
         net.backward_raw(dout, B, tag=tag)
         if self.allreduce is not None:
             self.allreduce(net.grad)
         self.optimizer.step(max_norm=self.clip_grad_norm)
+        self._after_step(st, idx, B, tag)
+
+    def _loss(self, st, idx, B, out, dout, tag):
+        """The loss launches of one minibatch: d loss / d out into dout, the minibatch's stats into the accumulators."""
+        stats = self.network._buf(tag + "stats", (8 + 4 * ((B + 255) // 256),))
+        C.jb_ppo_loss(int(self.continuous), ptr(out), ptr(idx), ptr(st["action"]), ptr(st["adv"]), ptr(st["ret"]),
+                      ptr(st["value"]), ptr(st["logp_old"]), B, self.action_size, self.network.nout, self.epsilon_clip,
+                      self.vf_coef, self.ent_coef, ptr(dout), ptr(stats), ptr(self._acc), stream_ptr())
+
+    def _after_step(self, st, idx, B, tag):
+        """Launches after the policy network's Adam: another network's or the multipliers' step (none for PPO)."""
 
     LAUNCHES_PER_MINIBATCH = 13   # take + in_fwd + gemm + heads + loss + finalize + 2 heads bwd + 3 gemm + sumsq + adam
     _GRAPH_INPUTS = ("state", "action", "adv", "ret", "value", "logp_old", "perm")   # rollout tensors a graph reads
 
     def _step_state(self):
-        """Every device tensor a minibatch step mutates (the graph warm-up saves and restores them)."""
-        return [self.network.flat, *self.optimizer.state_tensors(), self._acc, self._cursor]
+        """Every device tensor a minibatch step mutates (the graph warm-up saves and restores them): each optimiser's
+        parameters and state, and the learn accumulators."""
+        return ([t for opt in self._optimizers() for t in (opt.network.flat, *opt.state_tensors())]
+                + [self._acc, self._cursor])
 
     def _begin_epochs(self):
         """Device-side set-up before the optimisation epochs: the lr the graphs read and the learn accumulators."""
-        self.optimizer._sync_lr()          # graph replays do not pass through optimizer.step()'s host-side lr check
+        for opt in self._optimizers():
+            opt._sync_lr()             # graph replays do not pass through optimizer.step()'s host-side lr check
+        self._zero_acc()
+
+    def _zero_acc(self):
+        """_acc[0..2] and [5] sum from 0, [3] max_ratio from -inf, [4] min_prob from +inf."""
         self._acc.zero_()
         self._acc[3] = -float("inf")
         self._acc[4] = float("inf")
@@ -167,29 +182,13 @@ class PPO(BaseAgent):
             return g
         cur_idx = self.network._buf(f"mb{B}.cur_idx", (B,), torch.int32)
 
-        def chunk():
-            for _ in range(GRAPH_CHUNK):
-                C.jb_take_minibatch(ptr(st["perm"]), ptr(self._cursor), B, ptr(cur_idx), stream_ptr())
-                self._minibatch_step(st, cur_idx, B)
-
-        # warm-up on a side stream (allocates workspaces), restoring every mutated buffer afterwards
-        mutated = self._step_state()
-        saved = [t.clone() for t in mutated]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
+        def step():
             C.jb_take_minibatch(ptr(st["perm"]), ptr(self._cursor), B, ptr(cur_idx), stream_ptr())
             self._minibatch_step(st, cur_idx, B)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        for dst, src in zip(mutated, saved):
-            dst.copy_(src)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            chunk()
-        # capture does not execute, state is untouched
-        self._graphs[key] = graph
-        return graph
+
+        # the warm-up step restores every mutated buffer
+        g = self._graphs[key] = capture_after_warmup(step, restore=self._step_state(), repeat=GRAPH_CHUNK)
+        return g
 
     def _gae_reward(self, st, reward, next_state, N, T):
         """The reward jb_gae reads.  next_state: the N*T next-state rows when the caller has them, else None."""

@@ -26,13 +26,13 @@ import numpy as np
 import torch
 
 from ..buffer import EpisodeRing, RolloutBuffer
-from ..dev import C, ptr, require_cuda, stream_ptr
+from ..dev import C, capture_after_warmup, ptr, require_cuda, stream_ptr
 from ..network import Network
 from ..optimizer import Optimizer
 from .base import BaseAgent
+from .ppo import MAX_ACTION_SIZE
 
 CHUNK_ROWS = 8192        # rows per chunk step: ~16 MB per activation at hidden_size 512; not tuned
-MAX_ACTION_SIZE = {"discrete": 18, "continuous": 8}    # csrc/ppo_rowmath.cuh MAX_A_DISC / MAX_A
 
 
 class REINFORCE(BaseAgent):
@@ -147,20 +147,9 @@ class REINFORCE(BaseAgent):
         g = self._graphs.get(key)
         if g is not None:
             return g
-        # warm-up on a side stream (allocates workspaces), restoring every buffer a chunk step mutates
-        mutated = [self.network.grad, self._gsum, self._acc, self._cursor]
-        saved = [t.clone() for t in mutated]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            self._chunk_step(ring, w)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        for dst, src in zip(mutated, saved):
-            dst.copy_(src)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._chunk_step(ring, w)
+        # the warm-up restores every buffer a chunk step mutates
+        g = capture_after_warmup(lambda: self._chunk_step(ring, w),
+                                 restore=[self.network.grad, self._gsum, self._acc, self._cursor])
         self._graphs[key] = g
         return g
 

@@ -21,8 +21,6 @@ parameters with clip_grad_norm_ on the network's parameters only.
 
 The running statistics are not checkpointed, as for ICM-PPO.
 """
-import os
-
 import numpy as np
 import torch
 
@@ -30,33 +28,22 @@ from ..dev import C, ptr, stream_ptr
 from ..network.policy_value import ContinuousPolicyTwoValue, DiscretePolicyTwoValue
 from ..network.rnd import FEATURE, RND
 from ..optimizer import Optimizer
-from .base import cpu_state_dict
-from .curiosity import _RunningMeanStd, check_batch_norm_rows, load_two_adam_state, two_adam_state
-from .ppo import MAX_ACTION_SIZE, PPO
+from .curiosity import CuriosityPPO
+from .ppo import MAX_ACTION_SIZE
 
-RND_NETWORKS = {"rnd_mlp": "mlp", "rnd_cnn": "cnn"}       # RND network -> the policy head (observation kind) it pairs with
 TWO_VALUE_NETWORKS = {"discrete_policy_value": DiscretePolicyTwoValue, "continuous_policy_value": ContinuousPolicyTwoValue}
 
 
-class RND_PPO(PPO):
+class RND_PPO(CuriosityPPO):
     # rnd_next: the next-state rows the predictor reads; rnd_target: the cached target features
-    _GRAPH_INPUTS = PPO._GRAPH_INPUTS + ("value_i", "ret_i", "rnd_next", "rnd_target")
-    replicas_only = True          # parallel.attach: BatchNorm batch statistics and the running statistics are per replica
+    _GRAPH_INPUTS = CuriosityPPO._GRAPH_INPUTS + ("value_i", "ret_i", "rnd_next", "rnd_target")
     FAMILY = "RND-PPO"
-    needs_next_state = True       # RolloutCollector: keep every step's next state in the rollout
+    NETWORKS = {"rnd_mlp": "mlp", "rnd_cnn": "cnn"}
+    KEY = "rnd"
 
     def __init__(self, state_size, action_size, optim_config={"name": "adam"}, rnd_network="rnd_mlp", gamma_i=0.99,
                  extrinsic_coeff=2.0, intrinsic_coeff=1.0, obs_normalize=True, ri_normalize=True, batch_norm=True,
                  non_episodic=True, **kwargs):
-        if rnd_network not in RND_NETWORKS:
-            raise ValueError(f"RND-PPO: unknown rnd_network={rnd_network!r} (available: {', '.join(RND_NETWORKS)})")
-        head = kwargs.get("head", "mlp")
-        if RND_NETWORKS[rnd_network] != head:
-            raise ValueError(f"RND-PPO: rnd_network={rnd_network!r} takes the observations of head="
-                             f"{RND_NETWORKS[rnd_network]!r}, got head={head!r}")
-        if rnd_network == "rnd_cnn" and obs_normalize:
-            raise ValueError("RND-PPO: rnd_cnn needs obs_normalize=False; per-pixel observation normalisation of frames "
-                             "is not implemented")
         network = kwargs.get("network", "discrete_policy_value")
         if network not in TWO_VALUE_NETWORKS:
             raise ValueError(f"RND-PPO: network={network!r} has no two-value variant (available: "
@@ -65,62 +52,36 @@ class RND_PPO(PPO):
         if not 1 <= action_size <= max_a:
             raise ValueError(f"RND-PPO's {network.split('_')[0]} kernels take 1 to {max_a} actions, got "
                              f"action_size={action_size}")
-        kwargs["use_fused"] = False       # the persistent kernel computes PPO's loss only
-        super().__init__(state_size, action_size, optim_config=optim_config, **kwargs)
+        super().__init__(state_size, action_size, rnd_network, optim_config, extrinsic_coeff, intrinsic_coeff,
+                         obs_normalize, ri_normalize, batch_norm, **kwargs)
         self.network = TWO_VALUE_NETWORKS[network](state_size, action_size, D_hidden=kwargs.get("hidden_size", 512),
-                                                   head=head, device=self.device)
+                                                   head=kwargs.get("head", "mlp"), device=self.device)
         self.optimizer = Optimizer(**dict(optim_config), params=self.network.parameters())
-        self.gamma_i = float(gamma_i)
-        self.extrinsic_coeff, self.intrinsic_coeff = float(extrinsic_coeff), float(intrinsic_coeff)
-        self.obs_normalize, self.ri_normalize = bool(obs_normalize), bool(ri_normalize)
-        self.batch_norm, self.non_episodic = bool(batch_norm), bool(non_episodic)
-        D = int(np.prod(state_size))
+        self.gamma_i, self.non_episodic = float(gamma_i), bool(non_episodic)
         cnn = rnd_network == "rnd_cnn"
-        self.rnd = RND(state_size if cnn else D, batch_norm=self.batch_norm, device=self.device, seed=self.seed, cnn=cnn)
+        self.rnd = RND(state_size if cnn else int(np.prod(state_size)), batch_norm=self.batch_norm, device=self.device,
+                       seed=self.seed, cnn=cnn)
         self.rnd_optimizer = Optimizer(**dict(optim_config), params=self.rnd.parameters())
-        self.rms_obs = _RunningMeanStd((D,), self.device) if self.obs_normalize else None
-        self.rms_ri = _RunningMeanStd((1,), self.device)
-        self.rewems = None                # [N] reward-forward filter state, created at the first learn
         self._rnd_acc = torch.zeros(2, dtype=torch.float32, device=self.device)
         self._ri_mean = None
 
     # ----------------------------------------------------------------------------------- learn --
-    def _check_batch(self, NT):
-        check_batch_norm_rows(self.FAMILY, self.batch_norm, self.batch_size, NT)
-
-    def _rms(self):
-        return (self.rms_obs.mean, self.rms_obs.var) if self.obs_normalize else None
-
     def _intrinsic_reward(self, s_next, N, T):
         """Steps 1-4: r_i of every row, normalised when ri_normalize; fills the target cache."""
         NT = N * T
-        s_ = stream_ptr()
         pred = self.rnd.predictor
-        if self.obs_normalize:
-            D = self.rnd.D_in
-            part = pred._buf("rms.partials", (C.jb_col_partials_doubles(NT, D),), torch.float64)
-            C.jb_rms_update(ptr(s_next), NT, D, *(ptr(t) for t in self.rms_obs.tensors()), ptr(part), s_)
+        self._update_rms_obs(pred, s_next, NT)
         ri = pred._buf("pre.ri", (NT,))
         self.rnd.prepass(s_next, NT, self._rms(), ri)
         if not self.ri_normalize:
             return ri
-        if self.rewems is None or self.rewems.shape[0] != N:
-            self.rewems = torch.zeros(N, dtype=torch.float32, device=self.device)
-        out = pred._buf("pre.ri_hat", (NT,))
-        part = pred._buf("ri.partials", (C.jb_col_partials_doubles(NT, 1),), torch.float64)
-        C.jb_icm_reward(ptr(ri), ptr(ri), N, T, self.gamma_i, 1, ptr(self.rewems), *(ptr(t) for t in self.rms_ri.tensors()),
-                        ptr(part), ptr(pred._buf("pre.filt", (NT,))), 0.0, 1.0, ptr(out), s_)
-        return out
+        return self._filtered_reward(pred, "pre.ri_hat", ri, ri, N, T, self.gamma_i, 0.0, 1.0)
 
     def _advantages(self, st, state, action, reward, done, next_state, last_next_state, next_rows, N, T):
         net = self.network
         NT = N * T
         s = stream_ptr()
-        self._check_batch(NT)
-        s_next = next_state if next_state is not None else next_rows
-        if s_next is None:
-            raise ValueError("RND-PPO needs every step's next state (a rollout with next_state, or host transitions)")
-        st["rnd_next"] = s_next
+        s_next = st["rnd_next"] = self._next_rows(next_state if next_state is not None else next_rows, NT)
         ri = self._intrinsic_reward(s_next, N, T)
         st["rnd_target"] = self.rnd.target_cache(NT)
         self._ri_mean = ri.mean()
@@ -150,25 +111,21 @@ class RND_PPO(PPO):
                      int(self.use_standardization), ptr(st["adv"]), s)
         return st["ret"].mean()
 
-    def _minibatch_step(self, st, idx, B):
-        net = self.network
-        tag = f"mb{B}."
-        s_ = stream_ptr()
-        out = net.forward_raw(st["state"], idx, B, tag=tag)
-        dout = net._buf(tag + "dout", (B, net.nout))
-        stats = net._buf(tag + "stats", (8 + 4 * ((B + 255) // 256),))
+    def _loss(self, st, idx, B, out, dout, tag):
+        stats = self.network._buf(tag + "stats", (8 + 4 * ((B + 255) // 256),))
         C.jb_rnd_ppo_loss(int(self.continuous), ptr(out), ptr(idx), ptr(st["action"]), ptr(st["adv"]), ptr(st["ret"]),
                           ptr(st["value"]), ptr(st["ret_i"]), ptr(st["value_i"]), ptr(st["logp_old"]), B,
-                          self.action_size, net.nout, self.epsilon_clip, self.vf_coef, self.ent_coef, ptr(dout),
-                          ptr(stats), ptr(self._acc), s_)
-        net.backward_raw(dout, B, tag=tag)
-        self.optimizer.step(max_norm=self.clip_grad_norm)
+                          self.action_size, self.network.nout, self.epsilon_clip, self.vf_coef, self.ent_coef,
+                          ptr(dout), ptr(stats), ptr(self._acc), stream_ptr())
+
+    def _after_step(self, st, idx, B, tag):
         rtag = tag + "rnd."
         pred = self.rnd.predictor
         p = self.rnd.predict(st["rnd_next"], idx, B, self._rms(), rtag)
         dp = pred._buf(rtag + "dp", (B, FEATURE))
         rstats = pred._buf(rtag + "stats", (1 + (B + 7) // 8,))
-        C.jb_rnd_loss(ptr(p), ptr(st["rnd_target"]), ptr(idx), B, FEATURE, 0, ptr(dp), ptr(rstats), ptr(self._rnd_acc), s_)
+        C.jb_rnd_loss(ptr(p), ptr(st["rnd_target"]), ptr(idx), B, FEATURE, 0, ptr(dp), ptr(rstats), ptr(self._rnd_acc),
+                      stream_ptr())
         self.rnd.backward(dp, B, rtag)
         self.rnd_optimizer.step()
 
@@ -181,16 +138,6 @@ class RND_PPO(PPO):
         bn_f, bn_b = (3, 5) if self.batch_norm else (1, 1)
         trunk = (6, 9) if self.rnd.cnn else (0, 0)
         return 13 + 7 + bn_f + 6 + bn_b + 2 + sum(trunk)
-
-    def _step_state(self):
-        pred = self.rnd.predictor
-        return super()._step_state() + [pred.flat, *pred.buffer_tensors(), *self.rnd_optimizer.state_tensors(),
-                                        self._rnd_acc]
-
-    def _begin_epochs(self):
-        super()._begin_epochs()
-        self.rnd_optimizer._sync_lr()
-        self._rnd_acc.zero_()
 
     def _learn_result(self, mean_ret):
         v = torch.cat([self._acc[:6], mean_ret.view(1), self._rnd_acc, self._ri_mean.view(1)]).cpu().numpy()  # ONE read
@@ -205,21 +152,3 @@ class RND_PPO(PPO):
             "r_i": float(v[9]),
             "rnd_loss": float(v[7] / rcnt),
         }
-
-    def learning_rate_decay(self, step, optimizers=None, mode="cosine"):
-        super().learning_rate_decay(step, [self.optimizer, self.rnd_optimizer] if optimizers is None else optimizers, mode)
-
-    # ------------------------------------------------------------------------------ checkpoint --
-    # network / rnd / optimizer, the optimizer one torch-Adam layout over network.parameters() + the predictor's.
-    def save(self, path):
-        print(f"...Save model to {path}...")
-        ck = {"network": cpu_state_dict(self.network), "rnd": cpu_state_dict(self.rnd),
-              "optimizer": two_adam_state(self.optimizer, self.rnd_optimizer)}
-        torch.save(ck, os.path.join(path, "ckpt"))
-
-    def load(self, path):
-        print(f"...Load model from {path}...")
-        ck = torch.load(os.path.join(path, "ckpt"), map_location="cpu", weights_only=False)
-        self.network.load_state_dict(ck["network"])
-        self.rnd.load_state_dict(ck["rnd"])
-        load_two_adam_state(ck["optimizer"], self.optimizer, self.rnd_optimizer)

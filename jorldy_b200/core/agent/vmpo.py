@@ -19,11 +19,9 @@ import torch
 
 from ..dev import C, ptr, stream_ptr
 from ..optimizer import Optimizer
-from .base import cpu_optimizer_state, cpu_state_dict
-from .ddpg import _Scalar
+from .base import (_Scalar, cpu_state_dict, joint_optimizer_state, load_joint_optimizer_state, load_multipliers,
+                   multiplier_values)
 from .ppo import PPO
-
-MULTIPLIERS = ("eta", "alpha_mu", "alpha_sigma")
 
 
 class VMPO(PPO):
@@ -43,28 +41,22 @@ class VMPO(PPO):
         self.mult_optimizer = Optimizer(**dict(optim_config), params=self.mult.parameters())
 
     # ----------------------------------------------------------------------------------- learn --
-    def _minibatch_step(self, st, idx, B):
-        net = self.network
-        tag = f"mb{B}."
-        out = net.forward_raw(st["state"], idx, B, tag=tag)
-        dout = net._buf(tag + "dout", (B, net.nout))
-        stats = net._buf(tag + "vstats", (16 + 4 * ((B + 255) // 256),))
+    def _optimizers(self):
+        return [self.optimizer, self.mult_optimizer]
+
+    def _loss(self, st, idx, B, out, dout, tag):
+        stats = self.network._buf(tag + "vstats", (16 + 4 * ((B + 255) // 256),))
         C.jb_vmpo_loss(int(self.continuous), ptr(out), ptr(st["out"]), ptr(idx), ptr(st["action"]), ptr(st["adv"]),
-                       ptr(st["ret"]), B, self.action_size, net.nout, ptr(self.mult.flat), self.eps_eta,
+                       ptr(st["ret"]), B, self.action_size, self.network.nout, ptr(self.mult.flat), self.eps_eta,
                        self.eps_alpha_mu, self.eps_alpha_sigma, ptr(dout), ptr(self.mult.grad), ptr(stats),
                        ptr(self._acc), stream_ptr())
-        net.backward_raw(dout, B, tag=tag)
-        self.optimizer.step(max_norm=self.clip_grad_norm)
+
+    def _after_step(self, st, idx, B, tag):
         self.mult_optimizer.step()
         C.jb_vmpo_clamp(ptr(self.mult.flat), self.min_eta, self.min_alpha_mu, self.min_alpha_sigma, stream_ptr())
 
-    def _step_state(self):
-        return super()._step_state() + [self.mult.flat, *self.mult_optimizer.state_tensors()]
-
-    def _begin_epochs(self):
-        self.optimizer._sync_lr()
-        self.mult_optimizer._sync_lr()
-        self._acc.zero_()
+    def _zero_acc(self):
+        self._acc.zero_()         # all sums from 0: slot 4 counts the minibatches
 
     def _learn_result(self, mean_ret):
         v = torch.cat([self._acc[:5], mean_ret.view(1), self.mult.flat[:3]]).cpu().numpy()    # ONE device->host read
@@ -80,9 +72,6 @@ class VMPO(PPO):
             "mean_ret": float(v[5]),
         }
 
-    def learning_rate_decay(self, step, optimizers=None, mode="cosine"):
-        super().learning_rate_decay(step, [self.optimizer, self.mult_optimizer] if optimizers is None else optimizers, mode)
-
     # ------------------------------------------------------------------------------ checkpoint --
     def save(self, path):
         print(f"...Save model to {path}...")
@@ -97,43 +86,3 @@ class VMPO(PPO):
         load_joint_optimizer_state(ck["optimizer"], self.optimizer, self.mult_optimizer)
         load_multipliers(ck, self.mult)
 
-
-# One torch-Adam layout over network.parameters() + [eta, alpha_mu, alpha_sigma]: the multipliers are the three parameter
-# indices after the network's, each a 0-d tensor; their values are stored under their own names too.  V-MPO's and MPO's
-# checkpoints share it.
-def joint_optimizer_state(optimizer, mult_optimizer):
-    sd = cpu_optimizer_state(optimizer)
-    P = len(optimizer.network.p)
-    step = float(mult_optimizer._step_dev.item())
-    if step > 0:
-        m, v = mult_optimizer.exp_avg[:3].cpu(), mult_optimizer.exp_avg_sq[:3].cpu()
-        for k in range(3):
-            sd["state"][P + k] = {"step": torch.tensor(step), "exp_avg": m[k].clone(), "exp_avg_sq": v[k].clone()}
-    sd["param_groups"][0]["params"] = list(range(P + 3))
-    return sd
-
-
-def multiplier_values(mult):
-    vals = mult.flat[:3].cpu()
-    return {name: vals[k].clone() for k, name in enumerate(MULTIPLIERS)}
-
-
-def load_joint_optimizer_state(sd, optimizer, mult_optimizer):
-    P = len(optimizer.network.p)
-    st = sd.get("state", {})
-    get = lambda i: st[i] if i in st else st.get(str(i))
-    group = dict(sd["param_groups"][0], params=list(range(P)))
-    optimizer.load_state_dict({"state": {i: get(i) for i in range(P)} if st else {}, "param_groups": [group]})
-    mult_optimizer.param_groups[0]["lr"] = float(group["lr"])
-    if get(P) is not None:
-        for k in range(3):
-            e = get(P + k)
-            mult_optimizer.exp_avg[k].copy_(torch.as_tensor(e["exp_avg"]).reshape(()))
-            mult_optimizer.exp_avg_sq[k].copy_(torch.as_tensor(e["exp_avg_sq"]).reshape(()))
-        mult_optimizer._step_dev.fill_(int(float(get(P)["step"])))
-
-
-def load_multipliers(ck, mult):
-    for k, name in enumerate(MULTIPLIERS):
-        if name in ck:
-            mult.flat[k].copy_(torch.as_tensor(ck[name], dtype=torch.float32).reshape(()))

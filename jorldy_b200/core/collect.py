@@ -8,6 +8,7 @@ randomness).
 import torch
 
 from .buffer import DeviceRollout, EpisodeRing, FrameRollout, frame_store
+from .dev import capture_after_warmup
 
 
 class RolloutCollector:
@@ -50,17 +51,7 @@ class RolloutCollector:
             self._collect_eager()
             return self.rollout
         if self._graph is None:
-            # warm-up (allocates workspaces) on a side stream, then capture the T-step sequence
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._collect_eager()
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._collect_eager()
-            self._graph = g
+            self._graph = capture_after_warmup(self._collect_eager)      # the T-step sequence
         self._graph.replay()
         self.rollout.t = self.T
         return self.rollout
@@ -101,17 +92,7 @@ class EpisodeCollector:
             self._collect_eager()
             return self.ring
         if self._graph is None:
-            # warm-up on a side stream (allocates workspaces; its steps are real ones), then capture the round
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._collect_eager()
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._collect_eager()
-            self._graph = g
+            self._graph = capture_after_warmup(self._collect_eager)      # the warm-up's steps are this round's
             return self.ring
         self._graph.replay()
         return self.ring

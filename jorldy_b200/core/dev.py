@@ -10,6 +10,25 @@ def stream_ptr():
     return torch.cuda.current_stream().cuda_stream
 
 
+def capture_after_warmup(fn, restore=(), repeat=1):
+    """A CUDA graph of `repeat` calls of fn().  fn() first runs once eagerly on a side stream, which allocates its
+    workspaces; the tensors in `restore` then get back the values they had before it.  Capture does not execute."""
+    saved = [t.clone() for t in restore]
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+    for dst, src in zip(restore, saved):
+        dst.copy_(src)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        for _ in range(repeat):
+            fn()
+    return graph
+
+
 def ptr(t):
     return 0 if t is None else t.data_ptr()
 

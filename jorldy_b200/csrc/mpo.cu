@@ -24,6 +24,7 @@ using jbppo::MAX_A;
 using jbppo::MAX_A_DISC;
 using jbppo::log_softmax_row;
 using jbppo::atanh_clamped;
+using jbppo::block_sum;
 
 constexpr int MPO_THREADS = 256;
 constexpr int MPO_TARGET_THREADS = 512;   // 16 warps, one window per warp at a time
@@ -187,26 +188,6 @@ mpo_critic_target_kernel(const float* __restrict__ tq, const float* __restrict__
   }
 }
 
-template <int NV>
-__device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float x = v[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
-    if (lane == 0) smem[q * 32 + warp] = x;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float t = 0.f;
-    for (int w = 0; w < nw; ++w) t += smem[q * 32 + w];
-    v[q] = t;
-  }
-  __syncthreads();
-}
-
 // One thread per state row s = b n + t (target row b (n + 1) + t).  part = [eta-free log-mean-exp (discrete: the
 // log-partition under pi'), its d / d eta, L_pi row, KL_mu row, KL_sigma row].
 template <bool CONT, int NA>
@@ -324,7 +305,7 @@ mpo_policy_kernel(const float* __restrict__ out, const float* __restrict__ tout,
       part[2] = lpi; part[3] = km; part[4] = ks;
     }
   }
-  block_sum<MPO_PARTS>(part, sred);
+  block_sum<MPO_PARTS, MPO_THREADS / 32>(part, sred);
   if (threadIdx.x == 0) {
     float* p = partials + MPO_PARTS * blockIdx.x;
 #pragma unroll

@@ -232,10 +232,11 @@ __device__ __forceinline__ void logp_continuous(const float* o, int A, const flo
   }
 }
 
-// fixed-order block reduction of NV values; result broadcast to all threads
-template <int NV>
+// fixed-order block reduction of NV values; result broadcast to all threads.  NW: the warp count when the caller's block
+// size is a compile-time constant (0: read it from blockDim).
+template <int NV, int NW = 0>
 __device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = NW ? NW : (blockDim.x + 31) >> 5;
 #pragma unroll
   for (int q = 0; q < NV; ++q) {
     float x = v[q];

@@ -26,6 +26,7 @@ using jbppo::MAX_A;
 using jbppo::MAX_A_DISC;
 using jbppo::log_softmax_row;
 using jbppo::atanh_clamped;
+using jbppo::block_sum;
 
 constexpr int VMPO_THREADS = 256;
 constexpr int VMPO_SCALARS = 8;        // stats[8..15]: the minibatch scalars CTA 0 publishes for the finalize launch
@@ -42,27 +43,6 @@ __device__ __forceinline__ float key_value(uint32_t k) {
 
 __device__ __forceinline__ float row_adv(const float* __restrict__ adv, const int32_t* __restrict__ idx, int b) {
   return adv[idx ? idx[b] : b];
-}
-
-// fixed-order block sum of NV values; result broadcast to all threads
-template <int NV>
-__device__ __forceinline__ void block_sum(float* v, float* smem /*[NV][32]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float x = v[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
-    if (lane == 0) smem[q * 32 + warp] = x;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int q = 0; q < NV; ++q) {
-    float t = 0.f;
-    for (int w = 0; w < nw; ++w) t += smem[q * 32 + w];
-    v[q] = t;
-  }
-  __syncthreads();
 }
 
 // Exact k-th smallest (0-based) of the B advantages: four-bit radix select from the top digit down.  Each pass counts,
@@ -215,7 +195,7 @@ vmpo_loss_kernel(const float* __restrict__ out, const float* __restrict__ out_ol
   float M = sred[0];
   for (int w = 1; w < (int)(blockDim.x >> 5); ++w) M = fmaxf(M, sred[w]);
   __syncthreads();
-  block_sum<1>(cnt, sred);
+  block_sum<1, VMPO_THREADS / 32>(cnt, sred);
   const float n = cnt[0];
   float es[2] = {0.f, 0.f};
   if (n > 0.f) {
@@ -224,7 +204,7 @@ vmpo_loss_kernel(const float* __restrict__ out, const float* __restrict__ out_ol
       if (a > m) { const float z = a / eta; const float e = expf(z - M); es[0] += e; es[1] += e * (M - z); }
     }
   }
-  block_sum<2>(es, sred);
+  block_sum<2, VMPO_THREADS / 32>(es, sred);
   const float S = es[0];
 
   // ---- phase 3: this CTA's rows ---------------------------------------------------------------------------------
@@ -245,7 +225,7 @@ vmpo_loss_kernel(const float* __restrict__ out, const float* __restrict__ out_ol
     part[0] = w > 0.f ? w * logpi : 0.f;
     part[1] = km; part[2] = ks; part[3] = sq;
   }
-  block_sum<4>(part, sred);
+  block_sum<4, VMPO_THREADS / 32>(part, sred);
   if (threadIdx.x == 0) {
     float* sp = stats + VMPO_PARTIALS + 4 * blockIdx.x;
     sp[0] = part[0]; sp[1] = part[1]; sp[2] = part[2]; sp[3] = part[3];
