@@ -589,4 +589,65 @@ JB_API int jb_r2d2_loss(const float* q, const float* q_next, const float* qt_nex
                         const float* done, const double* weights, int B, int T, int A, int n_step, float gamma, float alpha,
                         float eta, float* dq, double* prio, float* stats, double* scratch, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * MuZero (Schrittwieser et al., arXiv:1911.08265) on flat observations, csrc/muzero.cu.  h(x) = sign(x)(sqrt(|x| + 1) - 1)
+ * + 1e-3 x; a support of V has the 2V + 1 integer atoms -V..V (1 <= V <= 300).  One warp per row / env / (window,
+ * position), fixed-order sums, no atomics: every entry point is bit-reproducible.
+ *   jb_muzero_scale_fwd   y [M, H] = (x - min) / max(max - min, 1e-5) per row (H <= 256); also into y2 [M, ld2] if not NULL.
+ *   jb_muzero_scale_bwd   dx of that map from x and dy: dy / s, plus d min at the argmin and d max at the argmax (lowest
+ *                         index on ties); with the range clamped, s is a constant and d max = 0.
+ *   jb_muzero_support_to_scalar  out [M] = h^-1(sum_i softmax(logits)_i (i - V)), logits [M, 2V + 1].
+ *   jb_muzero_scalar_to_support  out [M, 2V + 1] = two-hot of clamp(h(x), -V, V) on the integer atoms.
+ *   Search trees: one per env, S + 1 nodes of A edges (1 <= A <= 18), index e = (env (S + 1) + node) A + action.  An edge
+ *   holds edge_n (int32), edge_w, edge_p, edge_r (f32) and edge_child (int32, -1: not expanded); latent [N, S + 1, Hs];
+ *   count [N] nodes in use; bounds [N, 2] the min and max backed-up Q; path [N, S + 1] the last walk's edges (node A + a),
+ *   path_len [N].
+ *   jb_mcts_root          priors = softmax(pi_logits [N, A]); training: (1 - frac) priors + frac Dirichlet(dir_alpha), the
+ *                         gamma draws injected (gamma_in f64 [N, A]) or drawn as Gamma(alpha + 1) U^(1/alpha) by
+ *                         Marsaglia-Tsang on the Philox subsequence (seed, env << 8 | a) at the row counter
+ *                         jb_next_row_ctr(row_ctr, env); resets the tree with latent0 [N, Hs] at node 0;
+ *                         root_value [N] (may be NULL) = support_to_scalar(v_logits [N, 2V + 1]).
+ *   jb_mcts_select        one walk per env from the root by pUCT (c1 = 1.25, c2 = 19652): Q = R + gamma W / N normalised
+ *                         by the bounds (when max > min), 0 on an unvisited edge, ties to the lowest action; writes the path,
+ *                         leaf_node / leaf_action [N] (the unexpanded edge) and dyn_in [N, Hs + A] = [latent, onehot(a)].
+ *   jb_mcts_expand_backup stores latent_new [N, Hs] and softmax(pi_logits) at node count[env], the scalar reward of
+ *                         r_logits [N, 2R + 1] on the leaf edge, and backs G = support_to_scalar(v_logits) up the path
+ *                         leaf first: W += G, N += 1, bounds <- R + gamma W / N, G = R + gamma G.
+ *   jb_mcts_act           pi [N, A] = N(a) / sum N at the root; root_value [N] (may be NULL) = sum_a (N R + gamma W) /
+ *                         sum N; action [N] int64: training samples N(a)^(1 / temperature[0]) with u_in f64 [N] or a
+ *                         Philox uniform at the row counter, else argmax N (lowest index on ties).
+ *   jb_muzero_loss        B windows of L = K + n_step + 1 steps: reward, done, root_value [B, L], policy [B, L, A];
+ *                         logits time-major: pi [K + 1, B, A], v [K + 1, B, 2V + 1], r [K, B, 2R + 1] (r[k - 1] predicts
+ *                         position k).  z_k = fold_{i = n-1..0} (r_{k+i} + (1 - d_{k+i}) gamma z) from root_value_{k+n};
+ *                         a position after a done in the window is absorbing: z = 0, no policy loss, and a reward target
+ *                         r_{k-1} only when position k - 1 is not absorbing.  loss = (1/B) sum_b w_b sum_k c_k
+ *                         (value_coef CE_v + CE_r [k >= 1] + CE_pi), c_0 = 1, c_k = 1/K; weights f64 [B] or NULL;
+ *                         d_pi, d_v, d_r its gradients (same layouts); prio [B] f64 (may be NULL) = |v_0 - z_0|^alpha;
+ *                         stats = {loss, value_loss, reward_loss, policy_loss}; scratch: 3 B (K + 1) doubles.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_muzero_scale_fwd(const float* x, int M, int H, float* y, float* y2, int ld2, void* stream);
+JB_API int jb_muzero_scale_bwd(const float* x, const float* dy, int M, int H, float* dx, void* stream);
+JB_API int jb_muzero_support_to_scalar(const float* logits, int M, int V, float* out, void* stream);
+JB_API int jb_muzero_scalar_to_support(const float* x, int M, int V, float* out, void* stream);
+JB_API int jb_mcts_root(const float* pi_logits, const float* v_logits, const float* latent0, int N, int A, int S, int Hs,
+                        int V, int training, float dir_alpha, float frac, const double* gamma_in, uint64_t seed,
+                        long long* row_ctr, int* edge_n, float* edge_w, float* edge_p, float* edge_r, int* edge_child,
+                        float* latent, int* count, float* bounds, int* path, int* path_len, float* root_value,
+                        void* stream);
+JB_API int jb_mcts_select(int N, int A, int S, int Hs, float gamma, int* edge_n, float* edge_w, float* edge_p,
+                          float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                          int* path_len, int* leaf_node, int* leaf_action, float* dyn_in, void* stream);
+JB_API int jb_mcts_expand_backup(const float* latent_new, const float* pi_logits, const float* v_logits,
+                                 const float* r_logits, int N, int A, int S, int Hs, int V, int R, float gamma,
+                                 const int* leaf_node, const int* leaf_action, int* edge_n, float* edge_w, float* edge_p,
+                                 float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                                 int* path_len, void* stream);
+JB_API int jb_mcts_act(int N, int A, int S, float gamma, int training, const float* temperature, const double* u_in,
+                       uint64_t seed, long long* row_ctr, const int* edge_n, const float* edge_w, const float* edge_r,
+                       int64_t* action, float* pi, float* root_value, void* stream);
+JB_API int jb_muzero_loss(const float* pi_logits, const float* v_logits, const float* r_logits, const float* reward,
+                          const float* done, const float* root_value, const float* policy, const double* weights, int B,
+                          int K, int n_step, int A, int V, int R, float gamma, float value_coef, float alpha, float* d_pi,
+                          float* d_v, float* d_r, double* prio, float* stats, double* scratch, void* stream);
+
 #endif /* JORLDY_B200_H */

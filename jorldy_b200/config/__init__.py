@@ -9,7 +9,8 @@ which follow the SAC-Discrete paper, and `config.vmpo.{cartpole,mountaincar,pend
 paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the ICM keys,
 `config.rnd_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the RND keys,
 `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows, and
-`config.reinforce.{cartpole,mountaincar,pendulum,mujoco}`, PPO's rows with the REINFORCE keys; an existing JORLDY config directory on sys.path takes precedence
+`config.reinforce.{cartpole,mountaincar,pendulum,mujoco}`, PPO's rows with the REINFORCE keys, and
+`config.muzero.{cartpole,mountaincar}`, this project's MuZero settings; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -298,6 +299,26 @@ def _mpo_config(env):
     return dict(env=env_d, agent=a, optim=dict(name="adam", lr=3e-4), train=tr)
 
 
+# MuZero (arXiv:1911.08265): this project's choices, not a reference config file; a JORLDY config directory on sys.path
+# takes precedence.  gamma, the unroll, the n-step return, the simulation count, the Dirichlet noise, PER alpha / beta
+# 1.0 and the value loss weight 0.25 are the paper's; the supports cover h(max |target|) of both envs (|z| <= 1 / (1 -
+# gamma) = 333 for rewards of magnitude <= 1, h(333) = 17.6 <= 20); the temperature steps sit at half and three quarters
+# of the run's learns (one per update_period steps).
+_MUZERO_KEYS = dict(name="muzero", hidden_size=128, latent_size=64, gamma=0.997, num_simulation=50, num_unroll=5,
+                    td_steps=10, value_support=20, reward_support=1, value_loss_coef=0.25, alpha=1.0, beta=1.0,
+                    uniform_sample_prob=1e-3, batch_size=128, buffer_size=100000, start_train_step=2000,
+                    clip_grad_norm=5.0, root_dirichlet_alpha=0.25, root_exploration_fraction=0.25,
+                    temperature_learns=(3125, 4688), lr_decay=True)
+_MUZERO_ENVS = ("cartpole", "mountaincar")
+
+
+def _muzero_config(env):
+    env_d = dict(name="cartpole", action_type="discrete", render=False) if env == "cartpole" else \
+        dict(name="mountain_car", render=False)
+    return dict(env=env_d, agent=dict(_MUZERO_KEYS), optim=dict(name="adam", lr=3e-4),
+                train=dict(_TRAIN_SMALL, eval_iteration=10, update_period=16, num_workers=8))
+
+
 def available():
     out = []
     for ag, envs in _AC_ENVS.items():
@@ -311,6 +332,7 @@ def available():
     out += [f"config.rnd_ppo.{e}" for e in _RND_PPO_ENVS]
     out += [f"config.mpo.{e}" for e in _MPO_ENVS]
     out += [f"config.reinforce.{e}" for e in _REINFORCE_ENVS]
+    out += [f"config.muzero.{e}" for e in _MUZERO_ENVS]
     return out
 
 
@@ -337,6 +359,8 @@ def load(config_path):
         d = _mpo_config(env)
     elif agent == "reinforce" and env in _REINFORCE_ENVS:
         d = _reinforce_config(env)
+    elif agent == "muzero" and env in _MUZERO_ENVS:
+        d = _muzero_config(env)
     elif agent in _AC_ENVS and env in _AC_ENVS[agent]:
         d = _ac_config(agent, env)
     elif agent == "sac_discrete" and env in ("cartpole", "atari"):

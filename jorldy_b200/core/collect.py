@@ -168,13 +168,17 @@ class SequenceAssembler:
     actor's (h0, c0) from before the step.  Only those snapshots are kept (at most ceil(L / store_period) + 1 of them),
     never an [N, L, H] history.  An emitted window holds every field as [N, L, ...] oldest step first, plus h0 / c0 [N, H]
     of its first step.
+
+    Other window layouts pass `fields` (kept for every step), `period` and `snapshot` (kept for a window's first step
+    only): MuZero's windows are emitted every step and keep only their first observation.
     """
 
     FIELDS = ("state", "action", "prev_action", "reset", "reward", "done")
 
-    def __init__(self, n_burn_in, seq_len, n_step):
+    def __init__(self, n_burn_in, seq_len, n_step, fields=FIELDS, period=None, snapshot=("h0", "c0")):
         self.L = int(n_burn_in) + int(seq_len) + int(n_step)
-        self.period = max(1, int(seq_len) // 2)
+        self.period = max(1, int(seq_len) // 2) if period is None else int(period)
+        self.fields, self.snapshot = tuple(fields), tuple(snapshot)
         self.hist, self.t, self.pos, self.snap = None, 0, 0, {}
 
     def starts_window(self):
@@ -184,10 +188,10 @@ class SequenceAssembler:
     def push(self, tr):
         if self.hist is None:
             self.hist = {k: torch.zeros((tr[k].shape[0], self.L) + tuple(tr[k].shape[1:]), dtype=tr[k].dtype,
-                                        device=tr[k].device) for k in self.FIELDS}
+                                        device=tr[k].device) for k in self.fields}
         if self.starts_window():
-            self.snap[self.t] = (tr["h0"].clone(), tr["c0"].clone())
-        for k in self.FIELDS:
+            self.snap[self.t] = tuple(tr[k].clone() for k in self.snapshot)
+        for k in self.fields:
             self.hist[k][:, self.pos].copy_(tr[k])
         self.pos = (self.pos + 1) % self.L
         self.t += 1
@@ -196,7 +200,7 @@ class SequenceAssembler:
             return None
         sel = torch.as_tensor([(self.pos + i) % self.L for i in range(self.L)], device=self.hist["reward"].device)
         out = {k: v.index_select(1, sel) for k, v in self.hist.items()}
-        out["h0"], out["c0"] = self.snap.pop(start)
+        out.update(zip(self.snapshot, self.snap.pop(start)))
         return out
 
 
@@ -210,11 +214,11 @@ class ReplayCollector:
         n = getattr(agent, "n_step", 1)
         apex = type(agent).__name__ == "ApeX"
         trajectory = getattr(agent, "trajectory_windows", False)      # MPO: whole windows with the behaviour log mu
-        # recurrent agents (R2D2) bring their own sequence assembler and frame store
+        # recurrent agents (R2D2) and MuZero bring their own sequence assembler and frame store
         self.sequences = getattr(agent, "sequence_assembler", None)
         self.assembler = NStepAssembler(n, apex, agent.gamma, trajectory) \
             if (n > 1 or apex or trajectory) and self.sequences is None else None
-        if apex or self.sequences is not None:
+        if (apex or self.sequences is not None) and hasattr(agent, "set_actor_epsilons"):
             agent.set_actor_epsilons(env.num_envs, total=max(agent.num_workers, env.num_envs, 2))
         env.reset_device()
         # Atari-shaped envs: every frame is pushed once and the replay stores frame references (buffer/frame_store.py)
