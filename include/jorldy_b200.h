@@ -88,6 +88,15 @@ JB_API int jb_frame_gather(const uint8_t* frames, const int64_t* first, const in
 JB_API int jb_im2col_u8_frames(const uint8_t* frames, const int64_t* first, const int64_t* head, int64_t frames_per_lane,
                                int n_lanes, const int64_t* refs, const int32_t* idx, int M, float* col, int32_t* status,
                                void* stream);
+/* MuZero's representation input: the same columns for an 8x84x84 input, col [M*20*20, 512], whose channels 4..7 are
+ * action planes.  Plane k is the constant __fdiv_rn((float)a, (float)num_actions), a = actions[row * 4 + k] (row =
+ * idx[i], or i), the action that produced stack frame k; a frame at or before its episode's first frame has an all-zero
+ * plane.  Bit-equal to jb_im2col_u8 over the gathered stack with the planes materialised as channels 4..7.  A
+ * non-resident reference writes zero rows (planes included) and sets *status = 1. */
+JB_API int jb_im2col_u8_frames_actions(const uint8_t* frames, const int64_t* first, const int64_t* head,
+                                       int64_t frames_per_lane, int n_lanes, const int64_t* refs, const int64_t* actions,
+                                       int num_actions, const int32_t* idx, int M, float* col, int32_t* status,
+                                       void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * PER sum-tree — jorldy/core/buffer/per_buffer.py:19-101.  tree is f64[2*capacity-1].

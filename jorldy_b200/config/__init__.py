@@ -10,7 +10,7 @@ paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujo
 `config.rnd_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the RND keys,
 `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows, and
 `config.reinforce.{cartpole,mountaincar,pendulum,mujoco}`, PPO's rows with the REINFORCE keys, and
-`config.muzero.{cartpole,mountaincar}`, this project's MuZero settings; an existing JORLDY config directory on sys.path takes precedence
+`config.muzero.{cartpole,mountaincar,atari}`, this project's MuZero settings; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -309,10 +309,22 @@ _MUZERO_KEYS = dict(name="muzero", hidden_size=128, latent_size=64, gamma=0.997,
                     uniform_sample_prob=1e-3, batch_size=128, buffer_size=100000, start_train_step=2000,
                     clip_grad_norm=5.0, root_dirichlet_alpha=0.25, root_exploration_fraction=0.25,
                     temperature_learns=(3125, 4688), lr_decay=True)
-_MUZERO_ENVS = ("cartpole", "mountaincar")
+_MUZERO_ENVS = ("cartpole", "mountaincar", "atari")
+# Atari frames (CNN representation over 4 frames + 4 action planes).  The paper's: gamma 0.997, K = 5, n = 10, S = 50,
+# the Dirichlet noise, PER alpha = beta = 1, the value loss weight 0.25, batch 1024.  This project's choices: Adam at
+# 3e-4 (the paper: SGD with momentum), the 1 M-window replay and 100 k warm-up steps of the other Atari replay configs,
+# hidden 512 / latent 256 flat-latent dynamics and prediction MLPs (the paper: a ResNet on 6x6 spatial latents), the
+# supports 20 / 1 of the flat configs, which cover the sign-clipped rewards (the paper's 300 / 300 are for unclipped
+# rewards), 32 envs with one learn every 8 rounds of env steps (3.75 M learns in the 30 M-step run), and the temperature
+# steps at half and three quarters of those learns.
+_MUZERO_ATARI_KEYS = dict(_MUZERO_KEYS, head="cnn", hidden_size=512, latent_size=256, batch_size=1024,
+                          buffer_size=1000000, start_train_step=100000, temperature_learns=(1875000, 2812500))
 
 
 def _muzero_config(env):
+    if env == "atari":
+        return dict(env=dict(_ATARI_ENV), agent=dict(_MUZERO_ATARI_KEYS), optim=dict(name="adam", lr=3e-4),
+                    train=dict(_TRAIN_ATARI, update_period=8, num_workers=32))
     env_d = dict(name="cartpole", action_type="discrete", render=False) if env == "cartpole" else \
         dict(name="mountain_car", render=False)
     return dict(env=env_d, agent=dict(_MUZERO_KEYS), optim=dict(name="adam", lr=3e-4),

@@ -1,4 +1,5 @@
-"""MuZero (Schrittwieser, Antonoglou, Hubert et al., arXiv:1911.08265) on flat observations and discrete actions.
+"""MuZero (Schrittwieser, Antonoglou, Hubert et al., arXiv:1911.08265) on flat observations or Atari frames, with
+discrete actions.
 
 act_device(state, training) for N envs, one tree per env (csrc/muzero.cu):
   1. initial inference: h over the N observations, then f over the root latents;
@@ -18,11 +19,20 @@ PERBuffer at its max priority.  One learn():
      logit gradients and the priorities |v_0 - z_0|^alpha;
   4. the backward in reverse order, with the gradient into each dynamics step's latent input scaled by 0.5;
   5. Adam with clip_grad_norm, then update_priorities; one device->host read of the results.
+
+Atari frames (head="cnn", state_size [4, 84, 84]), under the batched collector only: attach_frames() gives the agent a
+single-frame store (buffer/frame_store.py) sized by frames_per_window, and a per-lane history of the last 4 actions.
+h's input is the lane's newest stack plus 4 action planes (csrc/frame_ring.cu jb_im2col_u8_frames_actions, read
+straight from the ring).  An act roots the search at each lane's newest stack (reference (lane << 40) | (head - 1))
+with the history as it was before the act (step_inputs["prev_actions"]), then shifts the action into the history, all
+inside the act graph.  A window keeps its first step's frame reference under `state` and that step's prev_actions; a
+learn runs h through the same im2col over the B sampled windows and the trunk's backward after h's.
 """
 import numpy as np
 import torch
 
-from ..buffer import PERBuffer
+from ..buffer import PERBuffer, frame_store
+from ..buffer.frame_store import STACK, FrameActionRows
 from ..collect import SequenceAssembler
 from ..dev import C, capture_after_warmup, ptr, require_cuda, stream_ptr
 from ..network.muzero import MuZero as MuZeroNetwork
@@ -46,8 +56,16 @@ class MuZero(BaseAgent):
                  clip_grad_norm=5.0, root_dirichlet_alpha=0.25, root_exploration_fraction=0.25,
                  temperature_learns=(500000, 750000), run_step=1e6, lr_decay=True, num_workers=1, device=None,
                  seed=0, use_cuda_graph=True, **kwargs):
-        if head != "mlp" or not isinstance(state_size, (int, np.integer)):
-            raise NotImplementedError("MuZero runs on flat observations only: the CNN representation is not implemented")
+        frames = head == "cnn"
+        if frames:
+            shape = tuple(int(d) for d in np.atleast_1d(state_size))
+            if len(shape) != 3:
+                raise NotImplementedError(f"state_size {list(shape)}: MuZero's CNN representation takes frame stacks")
+            if shape[1:] != (84, 84) or shape[0] != STACK:
+                raise ValueError(f"state_size {list(shape)}: MuZero's CNN representation takes [{STACK}, 84, 84] frame "
+                                 f"stacks (stack_frame {STACK})")
+        elif head != "mlp" or not isinstance(state_size, (int, np.integer)):
+            raise NotImplementedError("MuZero takes flat observations with head='mlp', or frame stacks with head='cnn'")
         if action_type != "discrete":
             raise ValueError("MuZero plans over discrete actions only")
         if not 1 <= int(action_size) <= MAX_ACTION_SIZE["discrete"]:
@@ -56,7 +74,9 @@ class MuZero(BaseAgent):
             if int(v) < 1:
                 raise ValueError(f"{name} {v}: must be at least 1")
         self.device = require_cuda(device)
-        self.state_size, self.action_size, self.seed = int(state_size), int(action_size), int(seed)
+        self.frames_input = frames
+        self.state_size = shape if frames else int(state_size)
+        self.action_size, self.seed = int(action_size), int(seed)
         self.gamma, self.S, self.K, self.n_step = float(gamma), int(num_simulation), int(num_unroll), int(td_steps)
         self.V, self.R, self.value_loss_coef = int(value_support), int(reward_support), float(value_loss_coef)
         self.alpha, self.beta, self.clip_grad_norm = float(alpha), float(beta), clip_grad_norm
@@ -66,12 +86,13 @@ class MuZero(BaseAgent):
         self.run_step, self.lr_decay, self.num_workers = run_step, lr_decay, num_workers
         self.use_cuda_graph = use_cuda_graph
         self.network = MuZeroNetwork(self.state_size, self.action_size, hidden_size, latent_size, self.V, self.R,
-                                     device=self.device, seed=self.seed)
+                                     head=head, device=self.device, seed=self.seed)
         self.optimizer = Optimizer(**dict(optim_config), params=self.network.parameters())
         self.memory = PERBuffer(self.buffer_size, uniform_sample_prob, device=self.device, seed=self.seed)
         self.L = self.K + self.n_step + 1
         self.sequence_assembler = SequenceAssembler(0, self.K + 1, self.n_step, fields=WINDOW_FIELDS, period=1,
-                                                    snapshot=("state",))
+                                                    snapshot=("state", "prev_actions") if frames else ("state",))
+        self._frames = self._hist = None      # frames: the store and the lanes' last STACK actions (attach_frames)
         self.num_learn, self.time_t = 0, 0
         self.step_inputs = None
         self.world_size, self.allreduce = 1, None
@@ -89,6 +110,8 @@ class MuZero(BaseAgent):
         return TEMPERATURES[min(k, len(TEMPERATURES) - 1)]
 
     def _net_input(self, s):
+        if self.frames_input:
+            return s
         return s.to(torch.float32).reshape(s.shape[0], -1)
 
     def _search_state(self, M):
@@ -97,14 +120,20 @@ class MuZero(BaseAgent):
             A, S, H, Hs = self.action_size, self.S, self.network.D_hidden, self.network.Hs
             f = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=self.device)
             i = lambda *shape: torch.zeros(*shape, dtype=torch.int32, device=self.device)
-            st = self._search[M] = {
-                "x": f(M, self.state_size), "h1": f(M, H), "pre": f(M, Hs), "s": f(M, Hs), "hid": f(M, H),
+            i64 = lambda *shape: torch.zeros(*shape, dtype=torch.int64, device=self.device)
+            if self.frames_input:
+                x = {"refs": i64(M), "prev_actions": i64(M, STACK),
+                     "lane_bits": torch.arange(M, dtype=torch.int64, device=self.device) << frame_store.POS_BITS}
+            else:
+                x = {"x": f(M, self.state_size)}
+            st = self._search[M] = dict(x, **{
+                "h1": f(M, self.network.D_repr), "pre": f(M, Hs), "s": f(M, Hs), "hid": f(M, H),
                 "pi": f(M, A), "v": f(M, 2 * self.V + 1), "r": f(M, 2 * self.R + 1), "z": f(M, Hs + A),
                 "n": i(M, S + 1, A), "w": f(M, S + 1, A), "p": f(M, S + 1, A), "er": f(M, S + 1, A),
                 "child": i(M, S + 1, A), "latent": f(M, S + 1, Hs), "count": i(M), "bounds": f(M, 2),
                 "path": i(M, S + 1), "path_len": i(M), "leaf_node": i(M), "leaf_action": i(M),
                 "action": torch.zeros(M, dtype=torch.int64, device=self.device), "policy": f(M, A),
-                "root_value": f(M), "v0": f(M)}
+                "root_value": f(M), "v0": f(M)})
         return st
 
     def _tree(self, st):
@@ -115,7 +144,13 @@ class MuZero(BaseAgent):
         A, S, Hs, V, R, g = self.action_size, self.S, net.Hs, self.V, self.R, self.gamma
         ctr = self._row_counter(M)
         tree = self._tree(st)
-        net.represent(st["x"], st["h1"], st["pre"], st["s"])
+        if self.frames_input:       # the roots: each lane's newest stack and its last STACK actions
+            torch.add(st["lane_bits"], self._frames.head, out=st["refs"]).sub_(1)
+            st["prev_actions"].copy_(self._hist)
+            x = FrameActionRows(self._frames, st["refs"], st["prev_actions"], A)
+        else:
+            x = st["x"]
+        net.represent(x, st["h1"], st["pre"], st["s"], tag="a.")
         net.predict(st["s"], st["hid"], st["pi"], st["v"])
         C.jb_mcts_root(ptr(st["pi"]), ptr(st["v"]), ptr(st["s"]), M, A, S, Hs, V, int(training), self.dir_alpha,
                        self.dir_frac, ptr(self._inject_gamma), self.seed, ptr(ctr), *tree, ptr(st["v0"]), s_)
@@ -128,12 +163,22 @@ class MuZero(BaseAgent):
         C.jb_mcts_act(M, A, S, g, int(training), ptr(self._temp), ptr(self._inject_u), self.seed + 1, ptr(ctr),
                       ptr(st["n"]), ptr(st["w"]), ptr(st["er"]), ptr(st["action"]), ptr(st["policy"]),
                       ptr(st["root_value"]), s_)
+        if self.frames_input:
+            self._hist[:, :-1].copy_(st["prev_actions"][:, 1:])
+            self._hist[:, -1].copy_(st["action"])
 
     def act_device(self, state, training=True):
-        """state [N, D] device tensor -> (action int64 [N], search value f32 [N]); sets step_inputs."""
+        """state [N, D] device tensor -> (action int64 [N], search value f32 [N]); sets step_inputs.  On frames, state
+        is the collector's [N, 4, 84, 84] stacks, whose newest frames the attached store already holds: the roots are
+        read from the store."""
         M = state.shape[0]
         st = self._search_state(M)
-        st["x"].copy_(state.reshape(M, -1))
+        if self.frames_input:
+            if self._frames is None or M != self._frames.n:
+                raise RuntimeError("MuZero on frames acts on the lanes of the frame store that attach_frames() made: "
+                                   "run it under the batched collector (main --sync)")
+        else:
+            st["x"].copy_(state.reshape(M, -1))
         t = self.temperature()
         if t != self._temp_host:
             self._temp.fill_(t)
@@ -143,16 +188,21 @@ class MuZero(BaseAgent):
             key = (M, bool(training))
             graph = self._graphs.get(key)
             if graph is None:
+                restore = [self._row_counter(M)] + ([self._hist] if self.frames_input else [])
                 graph = self._graphs[key] = capture_after_warmup(lambda: self._search_eager(M, training),
-                                                                 restore=[self._row_counter(M)])
+                                                                 restore=restore)
             graph.replay()
         else:
             self._search_eager(M, training)
         self.step_inputs = {"root_value": st["root_value"], "policy": st["policy"]}
+        if self.frames_input:
+            self.step_inputs["prev_actions"] = st["prev_actions"]
         return st["action"], st["root_value"]
 
     @torch.no_grad()
     def act(self, state, training=True):
+        if self.frames_input:
+            raise NotImplementedError("MuZero on frames runs under the batched collector (main --sync) only")
         s = self._net_input(self._state_to_device(state))
         action, _ = self.act_device(s, training)
         return {"action": action.cpu().numpy().reshape(-1, 1)}
@@ -161,9 +211,17 @@ class MuZero(BaseAgent):
         """The search keeps no state across steps."""
 
     def attach_frames(self, env):
-        if getattr(env, "frame_stack", False):
-            raise NotImplementedError("MuZero on frame-stack envs is not implemented")
-        return None
+        """Frames: a single-frame store for `env`'s lanes, sized so that every frame a live window references stays
+        resident (frame_store.frames_per_window), and a zeroed action history per lane.  None on flat observations."""
+        stack = bool(getattr(env, "frame_stack", False))
+        if stack != self.frames_input:
+            raise ValueError("MuZero with head='cnn' needs a frame-stack env, and a frame-stack env needs head='cnn'")
+        if not stack:
+            return None
+        F = frame_store.frames_per_window(self.buffer_size, env.num_envs, self.L)
+        self._frames = frame_store.FrameStore(env.num_envs, F, self.device)
+        self._hist = torch.zeros(env.num_envs, STACK, dtype=torch.int64, device=self.device)
+        return self._frames
 
     def interact_callback(self, transition):
         """Single-process driver: the step goes through the same window assembler with N = its rows."""
@@ -180,7 +238,7 @@ class MuZero(BaseAgent):
         """Forward of one learn: h, K dynamics steps, f over the K + 1 latents.  Returns the workspace dict."""
         net, K, A, H, Hs = self.network, self.K, self.action_size, self.network.D_hidden, self.network.Hs
         b = lambda name, *shape: net._buf("t." + name, shape)
-        ws = {"x": x, "h1": b("h1", B, H), "pre": b("pre", (K + 1) * B, Hs), "s": b("s", (K + 1) * B, Hs),
+        ws = {"x": x, "h1": b("h1", B, net.D_repr), "pre": b("pre", (K + 1) * B, Hs), "s": b("s", (K + 1) * B, Hs),
               "z": b("z", K * B, Hs + A), "hidg": b("hidg", K * B, H), "r": b("r", K * B, 2 * self.R + 1),
               "hidf": b("hidf", (K + 1) * B, H), "pi": b("pi", (K + 1) * B, A), "v": b("v", (K + 1) * B, 2 * self.V + 1)}
         rows = lambda t, k: t[k * B:(k + 1) * B]
@@ -210,12 +268,18 @@ class MuZero(BaseAgent):
             C.jb_add_f32(ptr(rows(ds, k - 1)), ptr(ds_in), B * Hs, s_)
         net.scale_bwd(rows(ws["pre"], 0), rows(ds, 0), rows(dpre, 0))
         net.dynamics_bwd_weights(ws["z"], ws["hidg"], dpre[B:], d_r, dhidg)
-        net.represent_bwd(ws["x"], ws["h1"], rows(dpre, 0), b("dh1", B, H))
+        net.represent_bwd(ws["x"], ws["h1"], rows(dpre, 0), b("dh1", B, net.D_repr))
 
     def _learn_windows(self, batch, weights):
         """One unroll -> loss -> backward -> Adam on B windows; returns the priorities f64 [B]."""
         net, K, A, B = self.network, self.K, self.action_size, batch["reward"].shape[0]
-        x = self._net_input(batch["state"]).contiguous()
+        if self.frames_input:
+            if self._frames is None:
+                raise RuntimeError("these windows hold frame references but no frame store is attached")
+            x = FrameActionRows(self._frames, batch["state"].contiguous(), batch["prev_actions"].contiguous(),
+                                self.action_size)
+        else:
+            x = self._net_input(batch["state"]).contiguous()
         ws = self._unroll(x, batch["action"], B)
         w32 = {k: batch[k].to(torch.float32).contiguous() for k in ("reward", "done", "root_value", "policy")}
         d_pi, d_v, d_r = (net._buf("t.d" + k, tuple(ws[k].shape)) for k in ("pi", "v", "r"))
@@ -243,6 +307,8 @@ class MuZero(BaseAgent):
         self.memory.update_priorities(indices, prio)
         self._stats[4:6].copy_(stats_per[:2])
         st = self._stats.cpu().numpy()
+        if self._frames is not None:
+            self._frames.check()
         return {"loss": float(st[0]), "value_loss": float(st[1]), "reward_loss": float(st[2]),
                 "policy_loss": float(st[3]), "sampled_p": float(st[4]), "mean_p": float(st[5]),
                 "num_learn": self.num_learn}

@@ -7,7 +7,8 @@ own ring of `F` frames, and the replay's `state` / `next_state` fields hold int6
 PER tree do not change.
 
 PPO's frame rollout (`FrameRollout`) keeps its states on a frame store too: `frames_per_rollout(T)` sizes the ring, and
-`FrameRows` hands the CNN head a view of the referenced stacks whose conv1 im2col reads the ring directly.
+`FrameRows` hands the CNN head a view of the referenced stacks whose conv1 im2col reads the ring directly.  MuZero's
+windows reference their first stack: `frames_per_window` sizes the ring, and `FrameActionRows` adds the action planes.
 
 This module owns the format: the sizing of the rings, the reference encoding ((lane << 40) | absolute frame position),
 the push of one env step, the gather and conv1's im2col.  A reference whose frames have been overwritten is never
@@ -48,6 +49,17 @@ def frames_per_rollout(T):
     h0 + 2T, and every frame the rollout references lies in [h0 - 4, h0 + 2T): 2T + 4 frames, whatever the dones.  The
     next rollout's pushes start only after that read.  FrameStore (and jb_frame_push) need at least 8 frames."""
     return max(2 * int(T) + 4, 8)
+
+
+def frames_per_window(capacity, num_lanes, window):
+    """Ring length F per lane for a replay of `capacity` windows of `window` steps, each window referencing its first
+    step's stack, one window per lane and step (MuZero): 2 (ceil(C/N) + window) + 2.
+
+    A lane's live windows are its newest W = ceil(C/N).  The oldest starts at step t0 = T - window - (W - 1) (T: steps
+    pushed so far); its stack is the frame at position h(t0) - 1 and reaches back to h(t0) - 4.  Each of the T - t0 =
+    window + W - 1 steps since pushed at most 2 frames, so the head is at most h(t0) + 2 (window + W - 1) and every
+    referenced frame lies in the last 2 (window + W) + 2 positions, whatever the dones."""
+    return max(2 * (-(-int(capacity) // int(num_lanes)) + int(window)) + 2, 8)
 
 
 def store_bytes(capacity, num_lanes, n_step, margin=None):
@@ -164,6 +176,37 @@ class FrameRows:
         s = self.store
         C.jb_im2col_u8_frames(ptr(s.frames), ptr(s.first), ptr(s.head), s.F, s.n, ptr(self.refs), ptr(idx), M, ptr(col),
                               ptr(s.status), stream_ptr())
+        return col
+
+
+class FrameActionRows(FrameRows):
+    """FrameRows plus MuZero's action planes: the [M,8,84,84] inputs named by `refs` and `actions` (int64 [M,4], the
+    actions that produced each stack's four frames, oldest first; csrc/frame_ring.cu zeroes the planes of frames at or
+    before an episode's first frame).  im2col writes conv1's 512-column matrix, planes as channels 4..7."""
+
+    def __init__(self, store, refs, actions, num_actions):
+        super().__init__(store, refs)
+        self.actions, self.num_actions = actions, int(num_actions)
+
+    @property
+    def shape(self):
+        return (int(self.refs.shape[0]), 2 * STACK, 84, 84)
+
+    def __getitem__(self, rows):
+        if not isinstance(rows, slice):
+            raise TypeError("FrameActionRows supports row slices only")
+        return FrameActionRows(self.store, self.refs[rows], self.actions[rows], self.num_actions)
+
+    def im2col(self, idx, M, col):
+        if idx is not None and (idx.dtype != torch.int32 or not idx.is_contiguous()):
+            raise ValueError(f"expected contiguous int32 row indices, got {idx.dtype}")
+        a = self.actions
+        if a.dtype != torch.int64 or tuple(a.shape) != (int(self.refs.shape[0]), STACK) or not a.is_contiguous():
+            raise ValueError(f"expected contiguous int64 [{int(self.refs.shape[0])},{STACK}] actions, got {a.dtype} "
+                             f"{tuple(a.shape)}")
+        s = self.store
+        C.jb_im2col_u8_frames_actions(ptr(s.frames), ptr(s.first), ptr(s.head), s.F, s.n, ptr(self.refs), ptr(a),
+                                      self.num_actions, ptr(idx), M, ptr(col), ptr(s.status), stream_ptr())
         return col
 
 

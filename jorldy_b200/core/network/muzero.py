@@ -1,5 +1,7 @@
-"""MuZero's three networks on flat observations (Schrittwieser et al., arXiv:1911.08265), H = D_hidden, Hs = latent_size:
+"""MuZero's three networks (Schrittwieser et al., arXiv:1911.08265), H = D_hidden, Hs = latent_size:
   representation h:  x [D] -> H (ReLU) -> Hs, min-max scaled
+                     (head="cnn", D_in = (4, 84, 84): the 4 frames + 4 action planes [8, 84, 84] -> the CNN head's trunk
+                     (conv 8x8s4 -> 4x4s2 -> 3x3s1, ReLU each) -> 3136 -> Hs, min-max scaled)
   dynamics g:        [s, onehot(a)] [Hs + A] -> H (ReLU) -> next latent Hs (min-max scaled) and reward logits 2R + 1
   prediction f:      s [Hs] -> H (ReLU) -> policy logits A and value logits 2V + 1
 Every latent is scaled per row to [0, 1] as (s - min) / max(max - min, 1e-5) (jb_muzero_scale_fwd).
@@ -7,7 +9,10 @@ Every latent is scaled per row to [0, 1] as (s - min) / max(max - min, 1e-5) (jb
 Parameters, in state_dict order: `h.l1.weight [H, D]`, `h.l1.bias`, `h.l2.weight [Hs, H]`, `h.l2.bias`, `g.l1.weight
 [H, Hs + A]`, `g.l1.bias`, `g.s.weight [Hs, H]`, `g.s.bias`, `g.r.weight [2R + 1, H]`, `g.r.bias`, `f.l1.weight [H, Hs]`,
 `f.l1.bias`, `f.pi.weight [A, H]`, `f.pi.bias`, `f.v.weight [2V + 1, H]`, `f.v.bias`.  Weights are orthogonal (gain
-sqrt(2) before a ReLU, 0.01 for the policy, 1 otherwise), biases zero.
+sqrt(2) before a ReLU, 0.01 for the policy, 1 otherwise), biases zero.  With head="cnn", h's parameters are
+`head.conv1.weight [32, 8, 8, 8]`, `head.conv1.bias`, `head.conv2.*`, `head.conv3.*` (the CNN head's names and init) and
+`h.l.weight [Hs, 3136]`, `h.l.bias`, in place of h.l1 / h.l2.  D_repr is the width of h's hidden activation h1: H, or
+the trunk's 3136 features.
 
 The callers own the activation buffers: each method takes its inputs and outputs, so the learner can lay the K + 1 unroll
 steps out as one time-major block ([k * B + b] is step k of window b) and run f over all of them at once.  The backward
@@ -18,6 +23,7 @@ import torch
 from ..dev import C, ptr, stream_ptr
 from . import layers as L
 from .base import FlatNetwork, init_gain, orthogonal_
+from .head import CNNHead
 
 NARROW = 32         # heads of at most this many outputs use the row kernel (csrc/heads.cu); wider ones the GEMM
 
@@ -26,21 +32,33 @@ class MuZero(FlatNetwork):
     def __init__(self, D_in, D_out, D_hidden=128, latent_size=64, value_support=20, reward_support=1, head="mlp",
                  device=None, seed=None):
         super().__init__(device)
-        if head != "mlp" or not isinstance(D_in, int):
-            raise NotImplementedError("MuZero runs on flat observations only (head='mlp')")
-        D, A, H, Hs = int(D_in), int(D_out), int(D_hidden), int(latent_size)
+        A, H, Hs = int(D_out), int(D_hidden), int(latent_size)
+        if head == "cnn":
+            C_, Hh, Ww = (int(d) for d in D_in)
+            self.trunk = CNNHead((2 * C_, Hh, Ww))        # frames + one action plane per frame
+            D = (C_, Hh, Ww)
+            self.D_repr = self.trunk.D_head_out
+            h_specs = self.trunk.specs() + [("h.l.weight", (Hs, self.D_repr)), ("h.l.bias", (Hs,))]
+        elif head == "mlp" and isinstance(D_in, int):
+            self.trunk, D, self.D_repr = None, int(D_in), H
+            h_specs = [("h.l1.weight", (H, D)), ("h.l1.bias", (H,)), ("h.l2.weight", (Hs, H)), ("h.l2.bias", (Hs,))]
+        else:
+            raise NotImplementedError("MuZero takes flat observations with head='mlp' or frame stacks with head='cnn'")
         self.D_in, self.D_out, self.D_hidden, self.Hs = D, A, H, Hs
         self.V, self.R = int(value_support), int(reward_support)
         nv, nr = 2 * self.V + 1, 2 * self.R + 1
-        self._specs = [("h.l1.weight", (H, D)), ("h.l1.bias", (H,)), ("h.l2.weight", (Hs, H)), ("h.l2.bias", (Hs,)),
+        self._specs = h_specs + [
                        ("g.l1.weight", (H, Hs + A)), ("g.l1.bias", (H,)), ("g.s.weight", (Hs, H)), ("g.s.bias", (Hs,)),
                        ("g.r.weight", (nr, H)), ("g.r.bias", (nr,)), ("f.l1.weight", (H, Hs)), ("f.l1.bias", (H,)),
                        ("f.pi.weight", (A, H)), ("f.pi.bias", (A,)), ("f.v.weight", (nv, H)), ("f.v.bias", (nv,))]
         self._allocate()
         gen = torch.Generator().manual_seed(seed) if seed is not None else None
-        gains = {"h.l1": "relu", "h.l2": "linear", "g.l1": "relu", "g.s": "linear", "g.r": "linear", "f.l1": "relu",
-                 "f.pi": "policy", "f.v": "linear"}
+        h_gains = {"h.l": "linear"} if self.trunk is not None else {"h.l1": "relu", "h.l2": "linear"}
+        gains = dict(h_gains, **{"g.l1": "relu", "g.s": "linear", "g.r": "linear", "f.l1": "relu", "f.pi": "policy",
+                                 "f.v": "linear"})
         with torch.no_grad():
+            if self.trunk is not None:
+                self.trunk.init(self.p, gen)
             for name, gain in gains.items():
                 w = self.p[f"{name}.weight"]
                 w.copy_(orthogonal_(tuple(w.shape), init_gain(gain), gen))
@@ -61,11 +79,16 @@ class MuZero(FlatNetwork):
         L.linear_bwd_dx(dout, self.p[f"{name}.weight"], dh, relu_act=h, accumulate=accumulate)
 
     # ------------------------------------------------------------------------------------ forward --
-    def represent(self, x, h1, pre, s, s2=None):
-        """x [M, D] -> h1 [M, H], pre [M, Hs] (before scaling), s [M, Hs]; s2 (a column block with its own row stride,
-        e.g. the first dynamics input) receives s too."""
-        L.linear_fwd(x, *self._w("h.l1"), h1, relu=True)
-        L.linear_fwd(h1, *self._w("h.l2"), pre, relu=False)
+    def represent(self, x, h1, pre, s, s2=None, tag="t."):
+        """x [M, D] -> h1 [M, D_repr], pre [M, Hs] (before scaling), s [M, Hs]; s2 (a column block with its own row
+        stride, e.g. the first dynamics input) receives s too.  head="cnn": x is a FrameActionRows (buffer/frame_store.py)
+        and the trunk keeps its column matrices under `tag` for represent_bwd."""
+        if self.trunk is not None:
+            self.trunk.forward(self, x, None, h1.shape[0], tag, True, out=h1)
+            L.linear_fwd(h1, *self._w("h.l"), pre, relu=False)
+        else:
+            L.linear_fwd(x, *self._w("h.l1"), h1, relu=True)
+            L.linear_fwd(h1, *self._w("h.l2"), pre, relu=False)
         self.scale(pre, s, s2)
 
     def dynamics(self, z, hid, pre, s, r_logits, s2=None):
@@ -113,7 +136,12 @@ class MuZero(FlatNetwork):
         L.linear_bwd_dw(d_r, hid, self.g["g.r.weight"], self.g["g.r.bias"])
         L.linear_bwd_dw(dhid, z, self.g["g.l1.weight"], self.g["g.l1.bias"])
 
-    def represent_bwd(self, x, h1, dpre, dh1):
+    def represent_bwd(self, x, h1, dpre, dh1, tag="t."):
+        if self.trunk is not None:
+            L.linear_bwd_dw(dpre, h1, self.g["h.l.weight"], self.g["h.l.bias"])
+            L.linear_bwd_dx(dpre, self.p["h.l.weight"], dh1, relu_act=h1)
+            self.trunk.backward(self, dh1, h1.shape[0], tag)
+            return
         L.linear_bwd_dw(dpre, h1, self.g["h.l2.weight"], self.g["h.l2.bias"])
         L.linear_bwd_dx(dpre, self.p["h.l2.weight"], dh1, relu_act=h1)
         L.linear_bwd_dw(dh1, x, self.g["h.l1.weight"], self.g["h.l1.bias"])

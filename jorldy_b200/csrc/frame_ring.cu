@@ -16,7 +16,7 @@
 // are no longer resident (an overwritten slot) is never read: its output is zeroed and *status is set, for the host to
 // raise on.  At B = 32..512 the gather moves 0.9..14 MB and is launch-latency-bound.
 // PPO's frame rollout keeps its states on the same rings; im2col_u8_frames_kernel below writes conv1's column matrix
-// straight from them, with the gather's stack rule and residency check.
+// straight from them, with the gather's stack rule and residency check, and with MuZero's action planes appended.
 #include "common.cuh"
 
 namespace {
@@ -99,22 +99,30 @@ __global__ void frame_gather_kernel(const uint8_t* __restrict__ frames, const in
 // c*64 + ky*8 + kx) read straight from the ring: grid = (stack i, output row oy), 256 threads.  Four threads resolve the
 // stack's four source frames (the stack rule and residency check of frame_gather_kernel) into shared memory; then each
 // thread turns one 4-byte frame-row load into one 16-byte column store, five times: 20 x 64 float4 = 20 KB per CTA.
-constexpr int OUT = 20, KSZ = 8, STRIDE = 4, K4 = STACK * KSZ * KSZ / 4;
-constexpr int ROW_VEC = OUT * K4;                  // float4 of one output row oy of one stack
+// PLANES (MuZero's representation input): four more channels c = 4 + k, each the constant a_k / A, where a_k
+// (actions[row][k]) is the action that produced stack frame k; a frame at or before its episode's first frame was
+// produced by no action and gets an all-zero plane.  K = 512, ten column stores per thread, 40 KB per CTA.
+constexpr int OUT = 20, KSZ = 8, STRIDE = 4;
 
+template <bool PLANES>
 __global__ void __launch_bounds__(256) im2col_u8_frames_kernel(
     const uint8_t* __restrict__ frames, const int64_t* __restrict__ first, const int64_t* __restrict__ head, long long F,
-    int n_lanes, const int64_t* __restrict__ refs, const int32_t* __restrict__ idx, float* __restrict__ col,
-    int32_t* __restrict__ status) {
+    int n_lanes, const int64_t* __restrict__ refs, const int32_t* __restrict__ idx, const int64_t* __restrict__ actions,
+    int num_actions, float* __restrict__ col, int32_t* __restrict__ status) {
+  constexpr int K4 = (PLANES ? 2 : 1) * STACK * KSZ * KSZ / 4;
+  constexpr int ROW_VEC = OUT * K4;              // float4 of one output row oy of one stack
   __shared__ long long src[STACK];               // frame index lane * F + slot, or -1 when the stack is not resident
+  __shared__ float plane[STACK];
   const long long i = blockIdx.x;
   const int oy = blockIdx.y;
   if (threadIdx.x < STACK) {
     const int k = threadIdx.x;
-    const long long r = refs[idx ? idx[i] : i];
+    const long long row = idx ? idx[i] : i;
+    const long long r = refs[row];
     const long long lane = r >> POS_BITS, p = r & POS_MASK;
     bool ok = r >= 0 && lane < n_lanes;
     long long s = -1;
+    float a = 0.f;
     if (ok) {
       const long long h = head[lane];
       ok = p < h && p >= h - F;
@@ -124,9 +132,11 @@ __global__ void __launch_bounds__(256) im2col_u8_frames_kernel(
         ok = lo >= h - F && f <= p;
         const long long q = p - 3 + k > f ? p - 3 + k : f;
         s = ok ? lane * F + q % F : -1;
+        if (PLANES && ok && p - 3 + k > f) a = __fdiv_rn((float)actions[row * STACK + k], (float)num_actions);
       }
     }
     src[k] = s;
+    if (PLANES) plane[k] = a;
     if (!ok && k == 0 && oy == 0) *reinterpret_cast<volatile int32_t*>(status) = 1;
   }
   __syncthreads();
@@ -134,12 +144,17 @@ __global__ void __launch_bounds__(256) im2col_u8_frames_kernel(
   for (int q = threadIdx.x; q < ROW_VEC; q += blockDim.x) {
     const int ox = q / K4, k4 = q % K4;
     const int kx4 = k4 & 1, ky = (k4 >> 1) & (KSZ - 1), c = k4 >> 4;
-    const long long s = src[c];
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (s >= 0) {
-      const uchar4 u = *reinterpret_cast<const uchar4*>(frames + (size_t)s * FRAME + (oy * STRIDE + ky) * 84 +
-                                                         ox * STRIDE + 4 * kx4);
-      v = make_float4((float)u.x / 255.0f, (float)u.y / 255.0f, (float)u.z / 255.0f, (float)u.w / 255.0f);
+    if (PLANES && c >= STACK) {
+      const float a = plane[c - STACK];
+      v = make_float4(a, a, a, a);
+    } else {
+      const long long s = src[c];
+      if (s >= 0) {
+        const uchar4 u = *reinterpret_cast<const uchar4*>(frames + (size_t)s * FRAME + (oy * STRIDE + ky) * 84 +
+                                                           ox * STRIDE + 4 * kx4);
+        v = make_float4((float)u.x / 255.0f, (float)u.y / 255.0f, (float)u.z / 255.0f, (float)u.w / 255.0f);
+      }
     }
     out[q] = v;
   }
@@ -174,7 +189,19 @@ JB_API int jb_im2col_u8_frames(const uint8_t* frames, const int64_t* first, cons
   if (!frames || !first || !head || !refs || !col || !status || M <= 0 || n_lanes <= 0 ||
       frames_per_lane < 8 || (((uintptr_t)frames & 3) | ((uintptr_t)col & 15)))
     return JB_ERR_INVALID;
-  im2col_u8_frames_kernel<<<dim3(M, OUT), 256, 0, (cudaStream_t)stream>>>(frames, first, head, frames_per_lane, n_lanes,
-                                                                           refs, idx, col, status);
+  im2col_u8_frames_kernel<false><<<dim3(M, OUT), 256, 0, (cudaStream_t)stream>>>(
+      frames, first, head, frames_per_lane, n_lanes, refs, idx, nullptr, 0, col, status);
+  return jb_check_launch();
+}
+
+JB_API int jb_im2col_u8_frames_actions(const uint8_t* frames, const int64_t* first, const int64_t* head,
+                                       int64_t frames_per_lane, int n_lanes, const int64_t* refs, const int64_t* actions,
+                                       int num_actions, const int32_t* idx, int M, float* col, int32_t* status,
+                                       void* stream) {
+  if (!frames || !first || !head || !refs || !actions || !col || !status || M <= 0 || n_lanes <= 0 ||
+      num_actions <= 0 || frames_per_lane < 8 || (((uintptr_t)frames & 3) | ((uintptr_t)col & 15)))
+    return JB_ERR_INVALID;
+  im2col_u8_frames_kernel<true><<<dim3(M, OUT), 256, 0, (cudaStream_t)stream>>>(
+      frames, first, head, frames_per_lane, n_lanes, refs, idx, actions, num_actions, col, status);
   return jb_check_launch();
 }
