@@ -42,6 +42,25 @@ JB_API int jb_env_classic_step(int kind, double* phys, float* obs, int32_t* elap
                                uint64_t seed, uint64_t stream_base, int n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * TicTacToe against a uniform-random opponent, one thread per board (csrc/env_tictactoe.cu).  The reference's
+ * tictactoe source is not available: these rules are this project's.  boards int32 [n, 2] (bit c: the agent's / the
+ * opponent's mark on cell c); obs f32 [n, 18] (the agent's marks, then the opponent's); legal u8 [n, 9] (the empty
+ * cells of obs, written in place); elapsed = the agent's moves this episode.
+ * reset: empty board; the opponent opens with probability 1/2, on cell floor(9 u).
+ * step: an occupied cell or an action outside 0..8 forfeits (-1, done); a line of the agent's +1, done; else the
+ * opponent marks the k-th empty cell, k = floor(u n_empty): its line -1, done; a full board 0, done; else 0.
+ * Draws: Philox (seed, stream_base | env) at counter (episode << 4) | move (0: the opening, m: the reply to move m).
+ * action_kind: 0 int64, 1 int32.  stats (may be NULL): [2] floats, += {episodes finished, sum of their scores}.
+ * ------------------------------------------------------------------------------------------- */
+JB_API int jb_env_tictactoe_reset(int32_t* boards, float* obs, uint8_t* legal, int32_t* elapsed, int64_t* episode,
+                                  float* score, const uint8_t* mask, uint64_t seed, uint64_t stream_base, int n,
+                                  void* stream);
+JB_API int jb_env_tictactoe_step(int32_t* boards, float* obs, uint8_t* legal, int32_t* elapsed, int64_t* episode,
+                                 float* score, const void* action, int action_kind, float* next_obs, float* reward,
+                                 float* done, float* stats, int auto_reset, uint64_t seed, uint64_t stream_base, int n,
+                                 void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * GAE — jorldy/core/agent/ppo.py:95-110.  Arrays are [N,T] row-major f32.
  * next_value may be NULL: then V(s'_t) = value[:,t+1] and last_value[N] closes the row.
  * ------------------------------------------------------------------------------------------- */
@@ -625,6 +644,11 @@ JB_API int jb_r2d2_loss(const float* q, const float* q_next, const float* qt_nex
  *   jb_mcts_act           pi [N, A] = N(a) / sum N at the root; root_value [N] (may be NULL) = sum_a (N R + gamma W) /
  *                         sum N; action [N] int64: training samples N(a)^(1 / temperature[0]) with u_in f64 [N] or a
  *                         Philox uniform at the row counter, else argmax N (lowest index on ties).
+ *   jb_mcts_root_legal / jb_mcts_select_legal  the same with legal u8 [N, A] masking the root (board games): priors are
+ *                         the softmax over the legal logits (0 elsewhere), the noise is drawn and normalised over the
+ *                         legal actions only (each on its unmasked subsequence), and an illegal root action never wins the
+ *                         select's argmax; every action stays allowed below the root.  A row with no legal action is
+ *                         searched unmasked; an all-legal mask gives jb_mcts_root / jb_mcts_select bit for bit.
  *   jb_muzero_loss        B windows of L = K + n_step + 1 steps: reward, done, root_value [B, L], policy [B, L, A];
  *                         logits time-major: pi [K + 1, B, A], v [K + 1, B, 2V + 1], r [K, B, 2R + 1] (r[k - 1] predicts
  *                         position k).  z_k = fold_{i = n-1..0} (r_{k+i} + (1 - d_{k+i}) gamma z) from root_value_{k+n};
@@ -646,6 +670,15 @@ JB_API int jb_mcts_root(const float* pi_logits, const float* v_logits, const flo
 JB_API int jb_mcts_select(int N, int A, int S, int Hs, float gamma, int* edge_n, float* edge_w, float* edge_p,
                           float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
                           int* path_len, int* leaf_node, int* leaf_action, float* dyn_in, void* stream);
+JB_API int jb_mcts_root_legal(const float* pi_logits, const float* v_logits, const float* latent0, int N, int A, int S,
+                              int Hs, int V, int training, float dir_alpha, float frac, const double* gamma_in,
+                              uint64_t seed, long long* row_ctr, int* edge_n, float* edge_w, float* edge_p,
+                              float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                              int* path_len, float* root_value, const uint8_t* legal, void* stream);
+JB_API int jb_mcts_select_legal(int N, int A, int S, int Hs, float gamma, int* edge_n, float* edge_w, float* edge_p,
+                                float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                                int* path_len, int* leaf_node, int* leaf_action, float* dyn_in, const uint8_t* legal,
+                                void* stream);
 JB_API int jb_mcts_expand_backup(const float* latent_new, const float* pi_logits, const float* v_logits,
                                  const float* r_logits, int N, int A, int S, int Hs, int V, int R, float gamma,
                                  const int* leaf_node, const int* leaf_action, int* edge_n, float* edge_w, float* edge_p,

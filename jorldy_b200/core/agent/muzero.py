@@ -27,6 +27,11 @@ straight from the ring).  An act roots the search at each lane's newest stack (r
 with the history as it was before the act (step_inputs["prev_actions"]), then shifts the action into the history, all
 inside the act graph.  A window keeps its first step's frame reference under `state` and that step's prev_actions; a
 learn runs h through the same im2col over the B sampled windows and the trunk's backward after h's.
+
+Board games (env.legal, e.g. TicTacToe): attach_legal(legal u8 [N, A]) masks the search root, as in the paper: the
+root priors and noise cover the legal moves only and an illegal move is never selected at the root
+(jb_mcts_root_legal / jb_mcts_select_legal); the act graph reads the mask in place.  Below the root every action stays
+allowed.  Without a mask the search is unchanged.
 """
 import numpy as np
 import torch
@@ -93,6 +98,7 @@ class MuZero(BaseAgent):
         self.sequence_assembler = SequenceAssembler(0, self.K + 1, self.n_step, fields=WINDOW_FIELDS, period=1,
                                                     snapshot=("state", "prev_actions") if frames else ("state",))
         self._frames = self._hist = None      # frames: the store and the lanes' last STACK actions (attach_frames)
+        self._legal = None                    # board games: the env's legal moves u8 [N, A] (attach_legal)
         self.num_learn, self.time_t = 0, 0
         self.step_inputs = None
         self.world_size, self.allreduce = 1, None
@@ -152,10 +158,18 @@ class MuZero(BaseAgent):
             x = st["x"]
         net.represent(x, st["h1"], st["pre"], st["s"], tag="a.")
         net.predict(st["s"], st["hid"], st["pi"], st["v"])
-        C.jb_mcts_root(ptr(st["pi"]), ptr(st["v"]), ptr(st["s"]), M, A, S, Hs, V, int(training), self.dir_alpha,
-                       self.dir_frac, ptr(self._inject_gamma), self.seed, ptr(ctr), *tree, ptr(st["v0"]), s_)
+        root_args = (ptr(st["pi"]), ptr(st["v"]), ptr(st["s"]), M, A, S, Hs, V, int(training), self.dir_alpha,
+                     self.dir_frac, ptr(self._inject_gamma), self.seed, ptr(ctr), *tree, ptr(st["v0"]))
+        select_args = (M, A, S, Hs, g, *tree, ptr(st["leaf_node"]), ptr(st["leaf_action"]), ptr(st["z"]))
+        if self._legal is None:
+            C.jb_mcts_root(*root_args, s_)
+        else:
+            C.jb_mcts_root_legal(*root_args, ptr(self._legal), s_)
         for _ in range(S):
-            C.jb_mcts_select(M, A, S, Hs, g, *tree, ptr(st["leaf_node"]), ptr(st["leaf_action"]), ptr(st["z"]), s_)
+            if self._legal is None:
+                C.jb_mcts_select(*select_args, s_)
+            else:
+                C.jb_mcts_select_legal(*select_args, ptr(self._legal), s_)
             net.dynamics(st["z"], st["hid"], st["pre"], st["s"], st["r"])
             net.predict(st["s"], st["hid"], st["pi"], st["v"])
             C.jb_mcts_expand_backup(ptr(st["s"]), ptr(st["pi"]), ptr(st["v"]), ptr(st["r"]), M, A, S, Hs, V, R, g,
@@ -179,6 +193,8 @@ class MuZero(BaseAgent):
                                    "run it under the batched collector (main --sync)")
         else:
             st["x"].copy_(state.reshape(M, -1))
+        if self._legal is not None and M != self._legal.shape[0]:
+            raise RuntimeError(f"MuZero acts on {M} rows but the attached legal-move mask has {self._legal.shape[0]}")
         t = self.temperature()
         if t != self._temp_host:
             self._temp.fill_(t)
@@ -222,6 +238,16 @@ class MuZero(BaseAgent):
         self._frames = frame_store.FrameStore(env.num_envs, F, self.device)
         self._hist = torch.zeros(env.num_envs, STACK, dtype=torch.int64, device=self.device)
         return self._frames
+
+    def attach_legal(self, legal):
+        """Board games: `legal` u8 [N, A] (the env's, updated in place) masks the root of every later search.  The act
+        graphs captured before are dropped, so the next act captures one that reads this mask."""
+        if legal.dtype != torch.uint8 or legal.dim() != 2 or legal.shape[1] != self.action_size or not legal.is_cuda \
+                or not legal.is_contiguous():
+            raise ValueError(f"legal {tuple(legal.shape)} {legal.dtype}: MuZero takes a u8 [N, {self.action_size}] "
+                             "device mask")
+        self._legal = legal
+        self._graphs.clear()
 
     def interact_callback(self, transition):
         """Single-process driver: the step goes through the same window assembler with N = its rows."""

@@ -4,8 +4,10 @@ from collections import OrderedDict
 from .classic import Cartpole, Pendulum, MountainCar
 from .frames import SyntheticAtari, _ACTIONS
 from .synth import SyntheticControl, _DIMS
+from .tictactoe import TicTacToe
 
-env_dict = OrderedDict(cartpole=Cartpole, mountain_car=MountainCar, pendulum=Pendulum, synthetic_atari=SyntheticAtari)
+env_dict = OrderedDict(cartpole=Cartpole, mountain_car=MountainCar, pendulum=Pendulum, synthetic_atari=SyntheticAtari,
+                       tictactoe=TicTacToe)
 for _game in _ACTIONS:            # atari.py registers one class per game (Breakout, Pong, ...)
     env_dict[_game] = (lambda g: (lambda **kw: SyntheticAtari(name=g, **kw)))(_game)
 

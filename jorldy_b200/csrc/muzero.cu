@@ -166,6 +166,20 @@ __device__ __forceinline__ float lane_softmax(const float* __restrict__ z, int A
   return e / jb_warp_sum(e);
 }
 
+// this lane's action is legal at the root (lanes >= A: false); a row with no legal action counts every action legal
+__device__ __forceinline__ bool root_legal(const uint8_t* __restrict__ legal, int env, int A, int lane) {
+  const bool ok = lane < A && legal[(size_t)env * A + lane] != 0;
+  return __any_sync(0xffffffffu, ok) ? ok : lane < A;
+}
+
+// lane_softmax over the lanes with ok only (the others return 0)
+__device__ __forceinline__ float lane_softmax_masked(const float* __restrict__ z, bool ok, int lane) {
+  const float v = ok ? z[lane] : -INFINITY;
+  const float m = jb_warp_max(v);
+  const float e = ok ? expf(v - m) : 0.f;
+  return e / jb_warp_sum(e);
+}
+
 // Gamma(alpha) = Gamma(alpha + 1) U^(1/alpha), Gamma(alpha + 1) by Marsaglia-Tsang; draw i of this subsequence is
 // Philox counter (ctr << 16) + i, so the rejection loop only consumes its own subsequence
 __device__ __forceinline__ double gamma_draw(uint64_t seed, uint64_t stream, uint64_t ctr, double alpha) {
@@ -186,22 +200,33 @@ __device__ __forceinline__ double gamma_draw(uint64_t seed, uint64_t stream, uin
   return g * pow(u_boost, 1.0 / alpha);
 }
 
+// MASKED: legal u8 [N, A] masks the root.  Priors are the softmax over the legal logits (0 on an illegal action) and the
+// noise is drawn and normalised over the legal lanes only, each on the subsequence it has unmasked, so an all-legal mask
+// gives the unmasked priors bit for bit.  A row with no legal action is searched unmasked.
+template <bool MASKED>
 __global__ void __launch_bounds__(WARPS * 32)
 mcts_root_kernel(const float* __restrict__ pi_logits, const float* __restrict__ v_logits, const float* __restrict__ latent0,
                  int N, int A, int S, int Hs, int V, int training, float dir_alpha, float frac,
                  const double* __restrict__ gamma_in, uint64_t seed, long long* __restrict__ row_ctr, Tree t,
-                 float* __restrict__ root_value) {
+                 float* __restrict__ root_value, const uint8_t* __restrict__ legal) {
   const int env = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (env >= N) return;
-  float prior = lane_softmax(pi_logits + (size_t)env * A, A, lane);
+  bool ok = lane < A;
+  float prior;
+  if constexpr (MASKED) {
+    ok = root_legal(legal, env, A, lane);
+    prior = lane_softmax_masked(pi_logits + (size_t)env * A, ok, lane);
+  } else {
+    prior = lane_softmax(pi_logits + (size_t)env * A, A, lane);
+  }
   if (training) {
     const uint64_t ctr = lane_ctr(row_ctr, env, lane);
     double g = 0.0;
-    if (lane < A)
+    if (ok)
       g = gamma_in ? gamma_in[(size_t)env * A + lane]
                    : gamma_draw(seed, ((uint64_t)env << 8) | (uint64_t)lane, ctr, (double)dir_alpha);
     const double sum = jb_warp_sum_d(g);
-    if (lane < A) prior = (float)((1.0 - (double)frac) * (double)prior + (double)frac * (g / sum));
+    if (ok) prior = (float)((1.0 - (double)frac) * (double)prior + (double)frac * (g / sum));
   }
   const double v = support_expect(v_logits + (size_t)env * (2 * V + 1), V, lane);
   const size_t nodes = (size_t)env * (S + 1);
@@ -221,11 +246,15 @@ mcts_root_kernel(const float* __restrict__ pi_logits, const float* __restrict__ 
   }
 }
 
+// MASKED: at depth 0 an illegal action (legal u8 [N, A]) never wins the argmax; below the root every action is allowed
+template <bool MASKED>
 __global__ void __launch_bounds__(WARPS * 32)
 mcts_select_kernel(int N, int A, int S, int Hs, float gamma, Tree t, int* __restrict__ leaf_node,
-                   int* __restrict__ leaf_action, float* __restrict__ dyn_in) {
+                   int* __restrict__ leaf_action, float* __restrict__ dyn_in, const uint8_t* __restrict__ legal) {
   const int env = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (env >= N) return;
+  bool root_ok = lane < A;
+  if constexpr (MASKED) root_ok = root_legal(legal, env, A, lane);
   const size_t nodes = (size_t)env * (S + 1);
   const float qmin = t.bounds[2 * env], qmax = t.bounds[2 * env + 1];
   int node = 0, depth = 0, a = 0;
@@ -236,8 +265,9 @@ mcts_select_kernel(int N, int A, int S, int Hs, float gamma, Tree t, int* __rest
   }
   while (true) {
     const size_t base = (nodes + node) * A;
+    const bool ok = MASKED && depth == 0 ? root_ok : lane < A;
     float score = -INFINITY;
-    if (lane < A) {
+    if (ok) {
       const int n = t.n[base + lane];
       float q = 0.f;
       if (n > 0) {
@@ -248,7 +278,7 @@ mcts_select_kernel(int N, int A, int S, int Hs, float gamma, Tree t, int* __rest
                        (float)(n + 1);
       score = q + pb * t.p[base + lane];
     }
-    a = warp_argmax(score, lane < A ? lane : 32);
+    a = warp_argmax(score, ok ? lane : 32);
     if (lane == 0) t.path[nodes + depth] = node * A + a;
     ++depth;
     const int c = t.child[base + a];
@@ -458,30 +488,67 @@ JB_API int jb_muzero_scalar_to_support(const float* x, int M, int V, float* out,
   return jb_check_launch();
 }
 
+namespace {
+
+template <bool MASKED>
+int mcts_root(const float* pi_logits, const float* v_logits, const float* latent0, int N, int A, int S, int Hs, int V,
+              int training, float dir_alpha, float frac, const double* gamma_in, uint64_t seed, long long* row_ctr,
+              const Tree& t, float* root_value, const uint8_t* legal, void* stream) {
+  if (!pi_logits || !v_logits || !latent0 || !tree_ok(t) || N <= 0 || A < 1 || A > MZ_MAX_A || S < 1 || Hs <= 0 ||
+      V < 1 || V > MZ_MAX_SUPPORT || (training && !(dir_alpha > 0.f)) || (MASKED && !legal))
+    return JB_ERR_INVALID;
+  mcts_root_kernel<MASKED><<<warp_grid(N), WARPS * 32, 0, (cudaStream_t)stream>>>(
+      pi_logits, v_logits, latent0, N, A, S, Hs, V, training, dir_alpha, frac, gamma_in, seed, row_ctr, t, root_value,
+      legal);
+  return jb_check_launch();
+}
+
+template <bool MASKED>
+int mcts_select(int N, int A, int S, int Hs, float gamma, const Tree& t, int* leaf_node, int* leaf_action,
+                float* dyn_in, const uint8_t* legal, void* stream) {
+  if (!tree_ok(t) || !leaf_node || !leaf_action || !dyn_in || N <= 0 || A < 1 || A > MZ_MAX_A || S < 1 || Hs <= 0 ||
+      (MASKED && !legal))
+    return JB_ERR_INVALID;
+  mcts_select_kernel<MASKED><<<warp_grid(N), WARPS * 32, 0, (cudaStream_t)stream>>>(N, A, S, Hs, gamma, t, leaf_node,
+                                                                                     leaf_action, dyn_in, legal);
+  return jb_check_launch();
+}
+
+}  // namespace
+
 JB_API int jb_mcts_root(const float* pi_logits, const float* v_logits, const float* latent0, int N, int A, int S, int Hs,
                         int V, int training, float dir_alpha, float frac, const double* gamma_in, uint64_t seed,
                         long long* row_ctr, int* edge_n, float* edge_w, float* edge_p, float* edge_r, int* edge_child,
                         float* latent, int* count, float* bounds, int* path, int* path_len, float* root_value,
                         void* stream) {
   const Tree t{edge_n, edge_w, edge_p, edge_r, edge_child, latent, count, bounds, path, path_len};
-  if (!pi_logits || !v_logits || !latent0 || !tree_ok(t) || N <= 0 || A < 1 || A > MZ_MAX_A || S < 1 || Hs <= 0 ||
-      V < 1 || V > MZ_MAX_SUPPORT || (training && !(dir_alpha > 0.f)))
-    return JB_ERR_INVALID;
-  mcts_root_kernel<<<warp_grid(N), WARPS * 32, 0, (cudaStream_t)stream>>>(pi_logits, v_logits, latent0, N, A, S, Hs, V,
-                                                                           training, dir_alpha, frac, gamma_in, seed,
-                                                                           row_ctr, t, root_value);
-  return jb_check_launch();
+  return mcts_root<false>(pi_logits, v_logits, latent0, N, A, S, Hs, V, training, dir_alpha, frac, gamma_in, seed,
+                          row_ctr, t, root_value, nullptr, stream);
+}
+
+JB_API int jb_mcts_root_legal(const float* pi_logits, const float* v_logits, const float* latent0, int N, int A, int S,
+                              int Hs, int V, int training, float dir_alpha, float frac, const double* gamma_in,
+                              uint64_t seed, long long* row_ctr, int* edge_n, float* edge_w, float* edge_p,
+                              float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                              int* path_len, float* root_value, const uint8_t* legal, void* stream) {
+  const Tree t{edge_n, edge_w, edge_p, edge_r, edge_child, latent, count, bounds, path, path_len};
+  return mcts_root<true>(pi_logits, v_logits, latent0, N, A, S, Hs, V, training, dir_alpha, frac, gamma_in, seed,
+                         row_ctr, t, root_value, legal, stream);
 }
 
 JB_API int jb_mcts_select(int N, int A, int S, int Hs, float gamma, int* edge_n, float* edge_w, float* edge_p,
                           float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
                           int* path_len, int* leaf_node, int* leaf_action, float* dyn_in, void* stream) {
   const Tree t{edge_n, edge_w, edge_p, edge_r, edge_child, latent, count, bounds, path, path_len};
-  if (!tree_ok(t) || !leaf_node || !leaf_action || !dyn_in || N <= 0 || A < 1 || A > MZ_MAX_A || S < 1 || Hs <= 0)
-    return JB_ERR_INVALID;
-  mcts_select_kernel<<<warp_grid(N), WARPS * 32, 0, (cudaStream_t)stream>>>(N, A, S, Hs, gamma, t, leaf_node, leaf_action,
-                                                                             dyn_in);
-  return jb_check_launch();
+  return mcts_select<false>(N, A, S, Hs, gamma, t, leaf_node, leaf_action, dyn_in, nullptr, stream);
+}
+
+JB_API int jb_mcts_select_legal(int N, int A, int S, int Hs, float gamma, int* edge_n, float* edge_w, float* edge_p,
+                                float* edge_r, int* edge_child, float* latent, int* count, float* bounds, int* path,
+                                int* path_len, int* leaf_node, int* leaf_action, float* dyn_in, const uint8_t* legal,
+                                void* stream) {
+  const Tree t{edge_n, edge_w, edge_p, edge_r, edge_child, latent, count, bounds, path, path_len};
+  return mcts_select<true>(N, A, S, Hs, gamma, t, leaf_node, leaf_action, dyn_in, legal, stream);
 }
 
 JB_API int jb_mcts_expand_backup(const float* latent_new, const float* pi_logits, const float* v_logits,

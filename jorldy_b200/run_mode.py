@@ -33,6 +33,12 @@ def _agent_config(config, env, **extra):
     return cfg
 
 
+def _attach_legal(env, agent):
+    """Board games: an agent that masks illegal moves (MuZero) reads the env's legal-move mask in place."""
+    if hasattr(env, "legal") and hasattr(agent, "attach_legal"):
+        agent.attach_legal(env.legal)
+
+
 def _report(step, metrics, logger, env, t0):
     stat = metrics.get_statistics()
     ep, sc = env.stats.tolist()
@@ -52,6 +58,7 @@ def single_train(config_path, unknown):
     assert agent.action_type == env.action_type
     if config.train.load_path:
         agent.load(config.train.load_path)
+    _attach_legal(env, agent)
     logger = LogManager(config.env.name, config.train.id or config.agent.name, config.train.experiment)
     config_manager.dump(logger.path)
     metrics = MetricManager()
@@ -103,6 +110,7 @@ def sync_distributed_train(config_path, unknown):
     assert agent.action_type == env.action_type
     if config.train.load_path:
         agent.load(config.train.load_path)
+    _attach_legal(env, agent)
     if world > 1:
         from .core import parallel
         parallel.attach(agent, world)
@@ -164,6 +172,7 @@ def evaluate(config_path, unknown):
     agent = Agent(**_agent_config(config, env))
     assert config.train.load_path
     agent.load(config.train.load_path)
+    _attach_legal(env, agent)
     episode = 0
     state = env.reset()
     try:
