@@ -42,7 +42,7 @@ JB_API int jb_env_classic_step(int kind, double* phys, float* obs, int32_t* elap
                                uint64_t seed, uint64_t stream_base, int n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * TicTacToe against a uniform-random opponent, one thread per board (csrc/env_tictactoe.cu).  The reference's
+ * TicTacToe, one thread per board (csrc/env_tictactoe.cu), here against a uniform-random opponent.  The reference's
  * tictactoe source is not available: these rules are this project's.  boards int32 [n, 2] (bit c: the agent's / the
  * opponent's mark on cell c); obs f32 [n, 18] (the agent's marks, then the opponent's); legal u8 [n, 9] (the empty
  * cells of obs, written in place); elapsed = the agent's moves this episode.
@@ -59,6 +59,22 @@ JB_API int jb_env_tictactoe_step(int32_t* boards, float* obs, uint8_t* legal, in
                                  float* score, const void* action, int action_kind, float* next_obs, float* reward,
                                  float* done, float* stats, int auto_reset, uint64_t seed, uint64_t stream_base, int n,
                                  void* stream);
+/* The same env with a choice of opponent: 0 the uniform-random one above, 1 a perfect player, 2 self-play.
+ * best u16 [3^9] (required for 1, NULL otherwise): per position, indexed in base 3 from the side to move (digit c = 1
+ * for its mark on cell c, 2 for the other side's), the 9-bit mask of the moves that reach the negamax value.  The
+ * perfect player plays the k-th set bit of best[position], k = floor(u popcount), u the random opponent's draw at the
+ * same counter; it opens like the random one, and on a board stepped after its game ended (best 0) it takes any empty
+ * cell, as the random one does.  Self-play: boards / obs hold (side to move, other side); reset gives an
+ * empty board and draws nothing; step: a forfeit -1 to the mover, a line +1, a full board 0 (each done), then the sides
+ * swap, so next_obs is seen by the side that did not just move; elapsed counts plies; score is the first player's
+ * outcome.  Any other opponent, or best given with the wrong one, is -22. */
+JB_API int jb_env_tictactoe_reset_opp(int opponent, const uint16_t* best, int32_t* boards, float* obs, uint8_t* legal,
+                                      int32_t* elapsed, int64_t* episode, float* score, const uint8_t* mask,
+                                      uint64_t seed, uint64_t stream_base, int n, void* stream);
+JB_API int jb_env_tictactoe_step_opp(int opponent, const uint16_t* best, int32_t* boards, float* obs, uint8_t* legal,
+                                     int32_t* elapsed, int64_t* episode, float* score, const void* action,
+                                     int action_kind, float* next_obs, float* reward, float* done, float* stats,
+                                     int auto_reset, uint64_t seed, uint64_t stream_base, int n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * GAE — jorldy/core/agent/ppo.py:95-110.  Arrays are [N,T] row-major f32.

@@ -10,7 +10,7 @@ paper's multiplier settings, `config.icm_ppo.{cartpole,mountaincar,pendulum,mujo
 `config.rnd_ppo.{cartpole,mountaincar,pendulum,mujoco,atari}`, PPO's rows with the RND keys,
 `config.mpo.{cartpole,mountaincar,pendulum,mujoco}`, this project's MPO settings on SAC's replay rows, and
 `config.reinforce.{cartpole,mountaincar,pendulum,mujoco}`, PPO's rows with the REINFORCE keys, and
-`config.muzero.{cartpole,mountaincar,atari,tictactoe}`, this project's MuZero settings; an existing JORLDY config directory on sys.path takes precedence
+`config.muzero.{cartpole,mountaincar,atari,tictactoe,tictactoe_selfplay}`, this project's MuZero settings; an existing JORLDY config directory on sys.path takes precedence
 (manager/config_manager.py).
 """
 from types import SimpleNamespace
@@ -309,7 +309,7 @@ _MUZERO_KEYS = dict(name="muzero", hidden_size=128, latent_size=64, gamma=0.997,
                     uniform_sample_prob=1e-3, batch_size=128, buffer_size=100000, start_train_step=2000,
                     clip_grad_norm=5.0, root_dirichlet_alpha=0.25, root_exploration_fraction=0.25,
                     temperature_learns=(3125, 4688), lr_decay=True)
-_MUZERO_ENVS = ("cartpole", "mountaincar", "atari", "tictactoe")
+_MUZERO_ENVS = ("cartpole", "mountaincar", "atari", "tictactoe", "tictactoe_selfplay")
 # Atari frames (CNN representation over 4 frames + 4 action planes).  The paper's: gamma 0.997, K = 5, n = 10, S = 50,
 # the Dirichlet noise, PER alpha = beta = 1, the value loss weight 0.25, batch 1024.  This project's choices: Adam at
 # 3e-4 (the paper: SGD with momentum), the 1 M-window replay and 100 k warm-up steps of the other Atari replay configs,
@@ -332,6 +332,14 @@ def _muzero_config(env):
         d = _muzero_config("cartpole")
         d["env"] = dict(name="tictactoe", render=False)
         d["agent"].update(gamma=1.0, td_steps=5, value_support=1)
+        return d
+    if env == "tictactoe_selfplay":
+        # two-player self-play (the paper's training for board games): the agent plays both sides and its search and
+        # value targets alternate sides; td_steps 9, the longest game in plies, so with gamma 1 every value target is
+        # the game's outcome for the side to move
+        d = _muzero_config("tictactoe")
+        d["env"]["opponent"] = "self"
+        d["agent"].update(two_player=True, td_steps=9)
         return d
     env_d = dict(name="cartpole", action_type="discrete", render=False) if env == "cartpole" else \
         dict(name="mountain_car", render=False)

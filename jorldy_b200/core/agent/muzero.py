@@ -32,6 +32,15 @@ Board games (env.legal, e.g. TicTacToe): attach_legal(legal u8 [N, A]) masks the
 root priors and noise cover the legal moves only and an illegal move is never selected at the root
 (jb_mcts_root_legal / jb_mcts_select_legal); the act graph reads the mask in place.  Below the root every action stays
 allowed.  Without a mask the search is unchanged.
+
+Two-player zero-sum games (two_player=True, e.g. TicTacToe with opponent="self"): a step's reward and its stored search
+value are the mover's, and the players alternate every step.  The negamax backup, where each ply's value is negated
+to the parent's side, is then exactly the single-player backup with the discount negated, so the search and the loss
+run the unchanged kernels at -gamma:
+  - backup: q = r - gamma W / N, g <- r - gamma g (the pseudocode flips W to the parent's side at each ply instead);
+  - root value (jb_mcts_act): sum(N r - gamma W) / sum N, the value for the side to move;
+  - n-step value target (jb_muzero_loss): z = r_k - gamma r_{k+1} + ... + (-gamma)^n v_{k+n}, cut at the first done.
+The reward and policy targets and the priorities do not change, nor do windows, replay, checkpoints or the masked root.
 """
 import numpy as np
 import torch
@@ -60,7 +69,7 @@ class MuZero(BaseAgent):
                  uniform_sample_prob=1e-3, buffer_size=100000, batch_size=128, start_train_step=2000,
                  clip_grad_norm=5.0, root_dirichlet_alpha=0.25, root_exploration_fraction=0.25,
                  temperature_learns=(500000, 750000), run_step=1e6, lr_decay=True, num_workers=1, device=None,
-                 seed=0, use_cuda_graph=True, **kwargs):
+                 seed=0, use_cuda_graph=True, two_player=False, **kwargs):
         frames = head == "cnn"
         if frames:
             shape = tuple(int(d) for d in np.atleast_1d(state_size))
@@ -83,6 +92,8 @@ class MuZero(BaseAgent):
         self.state_size = shape if frames else int(state_size)
         self.action_size, self.seed = int(action_size), int(seed)
         self.gamma, self.S, self.K, self.n_step = float(gamma), int(num_simulation), int(num_unroll), int(td_steps)
+        self.two_player = bool(two_player)
+        self._discount = -self.gamma if self.two_player else self.gamma    # the search and loss kernels' gamma
         self.V, self.R, self.value_loss_coef = int(value_support), int(reward_support), float(value_loss_coef)
         self.alpha, self.beta, self.clip_grad_norm = float(alpha), float(beta), clip_grad_norm
         self.dir_alpha, self.dir_frac = float(root_dirichlet_alpha), float(root_exploration_fraction)
@@ -147,7 +158,7 @@ class MuZero(BaseAgent):
 
     def _search_eager(self, M, training):
         st, net, s_ = self._search_state(M), self.network, stream_ptr()
-        A, S, Hs, V, R, g = self.action_size, self.S, net.Hs, self.V, self.R, self.gamma
+        A, S, Hs, V, R, g = self.action_size, self.S, net.Hs, self.V, self.R, self._discount
         ctr = self._row_counter(M)
         tree = self._tree(st)
         if self.frames_input:       # the roots: each lane's newest stack and its last STACK actions
@@ -314,7 +325,7 @@ class MuZero(BaseAgent):
         stats = net._buf("t.lossstats", (4,))
         C.jb_muzero_loss(ptr(ws["pi"]), ptr(ws["v"]), ptr(ws["r"]), ptr(w32["reward"]), ptr(w32["done"]),
                          ptr(w32["root_value"]), ptr(w32["policy"]), ptr(weights), B, K, self.n_step, A, self.V, self.R,
-                         self.gamma, self.value_loss_coef, self.alpha, ptr(d_pi), ptr(d_v), ptr(d_r), ptr(prio),
+                         self._discount, self.value_loss_coef, self.alpha, ptr(d_pi), ptr(d_v), ptr(d_r), ptr(prio),
                          ptr(stats), ptr(scratch), stream_ptr())
         self._backward(ws, d_pi, d_v, d_r, B)
         if self.allreduce is not None:

@@ -39,6 +39,16 @@ def _attach_legal(env, agent):
         agent.attach_legal(env.legal)
 
 
+def _check_players(env, agent):
+    """A two-player env (TicTacToe self-play) needs an agent whose targets alternate sides (MuZero two_player=True),
+    and such an agent needs a two-player env: any other pairing would learn from values of the wrong sign."""
+    env_2p, agent_2p = getattr(env, "two_player", False), getattr(agent, "two_player", False)
+    if env_2p != agent_2p:
+        raise ValueError(f"{type(env).__name__} is {'a two-player' if env_2p else 'a single-agent'} env but "
+                         f"{type(agent).__name__} was built for {'two players' if agent_2p else 'a single agent'}: "
+                         "two-player self-play takes MuZero with two_player=True")
+
+
 def _report(step, metrics, logger, env, t0):
     stat = metrics.get_statistics()
     ep, sc = env.stats.tolist()
@@ -58,6 +68,7 @@ def single_train(config_path, unknown):
     assert agent.action_type == env.action_type
     if config.train.load_path:
         agent.load(config.train.load_path)
+    _check_players(env, agent)
     _attach_legal(env, agent)
     logger = LogManager(config.env.name, config.train.id or config.agent.name, config.train.experiment)
     config_manager.dump(logger.path)
@@ -110,6 +121,7 @@ def sync_distributed_train(config_path, unknown):
     assert agent.action_type == env.action_type
     if config.train.load_path:
         agent.load(config.train.load_path)
+    _check_players(env, agent)
     _attach_legal(env, agent)
     if world > 1:
         from .core import parallel
@@ -172,6 +184,7 @@ def evaluate(config_path, unknown):
     agent = Agent(**_agent_config(config, env))
     assert config.train.load_path
     agent.load(config.train.load_path)
+    _check_players(env, agent)
     _attach_legal(env, agent)
     episode = 0
     state = env.reset()
